@@ -16,20 +16,20 @@ No tensor is ever transposed/flattened: the reference's flat sample index env*H+
 a2c_common.py:33-40) and minibatch slices (datasets.py:75-82) are honoured as an index mapping --
 minibatch i = envs [i*mb/H, (i+1)*mb/H) x all t.  The whole update phase (mini_epochs x num_minibatches)
 is captured in one CUDA graph; no .item()/nonzero() host syncs remain inside an epoch.
+
+Config parsing of the shared keys, the train loop, the summaries, the multi-GPU stats sync and checkpoint I/O are in
+``a2c_base.A2CBase``, shared with the discrete agent.
 """
-import os
 import time
-from datetime import datetime
 
 import numpy as np
 import torch
 import torch.distributed as dist
 
 from . import ops
-from .common import (AdaptiveScheduler, IdentityScheduler, LinearScheduler, DefaultAlgoObserver, DefaultRewardsShaper,
-                     create_vec_env, make_summary_writer)
-from .dist_utils import PackedStatsSync
-from .model import B200Model, CompileTolerantModel, resolve_device
+from .a2c_base import A2CBase
+from .common import IdentityScheduler
+from .model import B200Model
 
 STATS_SYNC_MODES = ('pooled', 'broadcast')
 
@@ -47,31 +47,6 @@ def rescale_actions(low, high, action):
     d = (high - low) / 2.0
     m = (high + low) / 2.0
     return action * d + m
-
-
-class _MeterView:
-    """torch_ext.AverageMeter look-alike over the device-resident meter block (torch_ext.py:326-352)."""
-
-    def __init__(self, agent, slot):
-        self._a, self._slot = agent, slot
-
-    @property
-    def current_size(self):
-        return int(self._a._meter_host()[3])
-
-    def __len__(self):
-        return self.current_size
-
-    def get_mean(self):
-        return np.asarray([self._a._meter_host()[self._slot]], dtype=np.float32)
-
-    @property
-    def mean(self):
-        return torch.tensor([self._a._meter_host()[self._slot]], dtype=torch.float32)
-
-    def clear(self):
-        self._a.meter.zero_()
-        self._a._meter_cache = None
 
 
 class _Dataset:
@@ -101,186 +76,28 @@ class _Dataset:
         return d
 
 
-class A2CAgent(CompileTolerantModel):
+class A2CAgent(A2CBase):
     def __init__(self, base_name, params):
-        self.config = config = params['config']
-        # a2c_common.py:172-188: PBT runs carry the policy's index in the experiment name
-        pbt_str = f'_pbt_{config["pbt_idx"]:02d}' if config.get('population_based_training', False) else ''
-        self.experiment_name = config.get('full_experiment_name') or (config['name'] + pbt_str + datetime.now().strftime("_%d-%H-%M-%S"))
+        config = params['config']
         # options of A2CBase that change what a run does and are not built here: refuse, never ignore
         if config.get('epochs_between_resets', 0) > 0:
             raise NotImplementedError('epochs_between_resets (forced env resets, a2c_common.py:553-556)')
         if config.get('self_play_config') is not None or config.get('self_play', False):
             raise NotImplementedError('self-play (SelfPlayManager) is outside the B200 hot path')
-        config.setdefault('features', {})
-        self.algo_observer = config['features'].get('observer') or DefaultAlgoObserver()
-        self.algo_observer.before_init(base_name, config, self.experiment_name)
-        self.network_params = params['network']
         model_name = params.get('model', {}).get('name', 'continuous_a2c_logstd')
         if model_name != 'continuous_a2c_logstd':
             raise NotImplementedError(f"model '{model_name}': only continuous_a2c_logstd is on the B200 hot path")
-
-        self.multi_gpu = config.get('multi_gpu', False)
-        self.multi_gpu_sync_stats = config.get('multi_gpu_sync_stats', True)
-        mode = config.get('multi_gpu_sync_stats_mode', 'pooled')
-        if mode not in STATS_SYNC_MODES:
-            raise ValueError(f"multi_gpu_sync_stats_mode must be one of {STATS_SYNC_MODES}, got '{mode}'")
-        self.multi_gpu_sync_stats_mode = mode
-        self.local_rank = self.global_rank = 0
-        self.world_size = 1
-        if self.multi_gpu:
-            self.local_rank = int(os.getenv('LOCAL_RANK', '0'))
-            self.global_rank = int(os.getenv('RANK', '0'))
-            self.world_size = int(os.getenv('WORLD_SIZE', '1'))
-            config['device'] = 'cuda:' + str(self.local_rank)
-            torch.cuda.set_device(self.local_rank)
-            if not dist.is_initialized():
-                dist.init_process_group('nccl', rank=self.global_rank, world_size=self.world_size,
-                                        device_id=torch.device(config['device']))
-            if self.global_rank != 0:
-                config['print_stats'] = False
-        self.ppo_device = config.get('device', 'cuda:0')
-        if not str(self.ppo_device).startswith('cuda'):
-            raise RuntimeError("rl_games_b200.A2CAgent runs on CUDA only (device=%r): there is no CPU fallback" % self.ppo_device)
-        self.device_t = resolve_device(self.ppo_device)          # 'cuda' without an index = the current device
-        torch.cuda.set_device(self.device_t)
-
-        self.network_path = config.get('network_path', './nn/')
-        self.env_config = config.get('env_config', {})
-        self.num_actors = config['num_actors']
-        self.env_name = config['env_name']
-        self.env_info = config.get('env_info')
-        if self.env_info is None:
-            self.vec_env = create_vec_env(self.env_name, self.num_actors, **self.env_config)
-            self.env_info = self.vec_env.get_env_info()
-        else:
-            self.vec_env = config.get('vec_env', None)
-        self.value_size = self.env_info.get('value_size', 1)
-        self.observation_space = self.env_info['observation_space']
-        self.weight_decay = config.get('weight_decay', 0.0)
-        if config.get('use_action_masks', False):
-            raise NotImplementedError('action masks are a discrete-PPO feature')
-        self.has_central_value = config.get('central_value_config') is not None
-        if self.has_central_value:
-            raise NotImplementedError('central_value_config is served by rl_games_b200.agent_cv.A2CAgentCV: build the agent through '
-                                      'rl_games_b200.register(runner) / rl_games_b200.runner.continuous_agent, which pick it')
-        self.central_value_net = None
-        self.truncate_grads = config.get('truncate_grads', False)
-        self.save_freq = config.get('save_frequency', 0)
-        self.save_best_after = config.get('save_best_after', 100)
-        self.print_stats = config.get('print_stats', True)
-        self.name = base_name
-        self.ppo = config.get('ppo', True)
-        self.max_epochs = config.get('max_epochs', -1)
-        self.max_frames = max(config.get('max_frames', -1), config.get('max_steps', -1))
         self.stop_fn = config.get('stop_fn', None)
         if self.stop_fn is not None and not callable(self.stop_fn):
             raise ValueError(f"'stop_fn' must be callable, got {type(self.stop_fn).__name__}")
-
-        self.is_adaptive_lr = config['lr_schedule'] == 'adaptive'
-        self.linear_lr = config['lr_schedule'] == 'linear'
-        self.schedule_type = config.get('schedule_type', 'per_minibatch')
-        if self.schedule_type == 'legacy':
-            self.schedule_type = 'per_minibatch'
-        if self.is_adaptive_lr and self.schedule_type not in ('per_minibatch', 'standard'):
-            raise NotImplementedError("adaptive lr_schedule with schedule_type=%r: 'per_minibatch' (the default) and 'standard' "
-                                      "(one step per mini-epoch) run on the device scheduler" % self.schedule_type)
-        if self.is_adaptive_lr:
-            self.kl_threshold = config['kl_threshold']
-            self.scheduler = AdaptiveScheduler(self.kl_threshold, min_lr=config.get('min_lr', 1e-6),
-                                               max_lr=config.get('max_lr', 1e-2), lr_multiplier=config.get('lr_multiplier', 1.5))
-        elif self.linear_lr:
-            if self.max_epochs == -1 and self.max_frames == -1:
-                self.scheduler = IdentityScheduler()
-            else:
-                use_epochs = self.max_epochs != -1
-                self.scheduler = LinearScheduler(float(config['learning_rate']), min_lr=config.get('min_lr', 1e-6),
-                                                 max_steps=self.max_epochs if use_epochs else self.max_frames,
-                                                 use_epochs=use_epochs, apply_to_entropy=config.get('schedule_entropy', False),
-                                                 start_entropy_coef=config.get('entropy_coef'))
-        else:
-            self.scheduler = IdentityScheduler()
-
-        self.e_clip = config['e_clip']
-        self.clip_value = config['clip_value']
-        rs = config['reward_shaper']
-        self.rewards_shaper = rs if not isinstance(rs, dict) else DefaultRewardsShaper(**rs)
-        self.num_agents = self.env_info.get('agents', 1)
-        if self.num_agents != 1:
-            raise NotImplementedError('multi-agent envs are not on the B200 hot path yet')
-        self.autoreset_mode = (self.env_info or {}).get('autoreset_mode', 'same_step')
-        self.mask_autoreset_rows = self.autoreset_mode == 'next_step'
-        if self.mask_autoreset_rows and self.num_agents > 1:
-            raise ValueError("PPO next_step autoreset masking does not support multi-agent envs; "
-                             "wrap the env with a same_step autoreset adapter instead")
-        self.horizon_length = config['horizon_length']
-        self.seq_length = config.get('seq_length', 4)
-        self.normalize_advantage = config['normalize_advantage']
-        # EMA advantage normaliser (a2c_common.py:369, :473-475): GeneralizedMovingStats((1,), decay=adv_rms_momentum), 'mean_std'
-        self.normalize_rms_advantage = bool(config.get('normalize_rms_advantage', False)) and self.normalize_advantage
-        self.adv_rms_momentum = float(config.get('adv_rms_momentum', 0.5))
-        self.normalize_input = config['normalize_input']
-        self.normalize_value = config.get('normalize_value', False)
-        if type(self.observation_space).__name__ == 'Dict':
-            raise NotImplementedError('Dict observation spaces are not on the B200 hot path yet')
-        self.obs_shape = self.observation_space.shape
-        if len(self.obs_shape) != 1:
-            raise NotImplementedError('only flat observations are on the B200 hot path')
-        self.critic_coef = config['critic_coef']
-        self.grad_norm = config['grad_norm']
-        self.gamma = config['gamma']
-        self.tau = config['tau']
-        self.games_to_track = config.get('games_to_track', 100)
-        self.batch_size = self.horizon_length * self.num_actors * self.num_agents
-        self.batch_size_envs = self.horizon_length * self.num_actors
-        if 'minibatch_size' not in config and 'minibatch_size_per_env' not in config:
-            raise ValueError("Configuration must include either 'minibatch_size' or 'minibatch_size_per_env'. "
-                             "Neither was found in the provided config.")
-        self.minibatch_size_per_env = config.get('minibatch_size_per_env', 0)
-        self.minibatch_size = config.get('minibatch_size', self.num_actors * self.minibatch_size_per_env)
-        if self.minibatch_size <= 0:
-            raise ValueError(f"'minibatch_size' must be greater than 0. Calculated value: {self.minibatch_size}.")
-        self.num_minibatches = self.batch_size // self.minibatch_size
-        if self.batch_size % self.minibatch_size != 0:
-            raise ValueError(f"'batch_size' ({self.batch_size}) must be divisible by 'minibatch_size' ({self.minibatch_size}). "
-                             "Ensure that 'batch_size' is a multiple of 'minibatch_size'.")
-        if self.minibatch_size % self.horizon_length != 0:
-            raise NotImplementedError("minibatch_size must be a multiple of horizon_length on the B200 path "
-                                      "(minibatches are whole-env slices of the time-major arena)")
-        self.envs_per_mb = self.minibatch_size // self.horizon_length
-        self.mini_epochs_num = config['mini_epochs']
+        super().__init__(base_name, params)
+        self.network_path = config.get('network_path', './nn/')
         # None (key absent) = the reference's 'auto' (a2c_common.py:427-429): resolved once the model geometry is known
         self.mixed_precision = config.get('mixed_precision', None)
-        self.last_lr = float(config['learning_rate'])
-        self.frame = 0
-        self.update_time = self.play_time = 0
-        self.mean_rewards = self.last_mean_rewards = -float('inf')
-        self.epoch_num = 0
-        self.curr_frames = 0
-        self.train_dir = config.get('train_dir', 'runs')
-        self.experiment_dir = os.path.join(self.train_dir, self.experiment_name)
-        self.nn_dir = os.path.join(self.experiment_dir, 'nn')
-        self.summaries_dir = os.path.join(self.experiment_dir, 'summaries')
-        for d in (self.train_dir, self.experiment_dir, self.nn_dir, self.summaries_dir):
-            os.makedirs(d, exist_ok=True)
-        self.entropy_coef = config['entropy_coef']
-        self.writer = make_summary_writer(self.summaries_dir) if self.global_rank == 0 else None
-        self.value_bootstrap = config.get('value_bootstrap', True)
-        self.use_smooth_clamp = config.get('use_smooth_clamp', False)
         self.is_tensor_obses = False
         self.is_rnn = False
         self.rnn_states = None
         self.zero_rnn_on_done = config.get('zero_rnn_on_done', True)
-
-        # ---- ContinuousA2CBase (a2c_common.py:1484-1497) ----
-        self.is_discrete = False
-        action_space = self.env_info['action_space']
-        self.actions_num = action_space.shape[0]
-        self.bounds_loss_coef = config.get('bounds_loss_coef', None)
-        self.bound_loss_type = config.get('bound_loss_type', 'bound')
-        self.clip_actions = config.get('clip_actions', True)
-        self.actions_low = torch.from_numpy(np.asarray(action_space.low).copy()).float().to(self.device_t)
-        self.actions_high = torch.from_numpy(np.asarray(action_space.high).copy()).float().to(self.device_t)
 
         # ---- A2CAgent (a2c_continuous.py:27-76) ----
         self.model = B200Model(self.network_params, self.obs_shape[0], self.actions_num, self.device_t,
@@ -336,23 +153,62 @@ class A2CAgent(CompileTolerantModel):
         # NCCL all-reduces are stream-ordered and graph-capturable; opt-out knob for debugging
         self.graph_multi_gpu = bool(config.get('b200_cuda_graph_multi_gpu', True))
         self.rng_seed = int(config.get('b200_rng_seed', params.get('seed', 0) or 0)) + 7919 * self.global_rank
-        self._stats_snapshots = {}
         self._graph_update = None
         self._graph_epoch = None
-        self._meter_cache = None
-        self._tensors_ready = False
-        self.obs = None
         self.train_result = None
-        self.game_rewards = _MeterView(self, 0)
-        self.game_shaped_rewards = _MeterView(self, 1)
-        self.game_lengths = _MeterView(self, 2)
         self.algo_observer.after_init(self)
 
-    # =============================================================================== allocation
-    @property
-    def device(self):
-        return self.ppo_device
+    def _experiment_suffix(self, config):
+        # a2c_common.py:172-188: PBT runs carry the policy's index in the experiment name
+        return f'_pbt_{config["pbt_idx"]:02d}' if config.get('population_based_training', False) else ''
 
+    def _check_stats_sync_mode(self, mode):
+        if mode not in STATS_SYNC_MODES:
+            raise ValueError(f"multi_gpu_sync_stats_mode must be one of {STATS_SYNC_MODES}, got '{mode}'")
+        return mode
+
+    def _parse_config(self, config):
+        self.value_size = self.env_info.get('value_size', 1)
+        self.observation_space = self.env_info['observation_space']
+        if config.get('use_action_masks', False):
+            raise NotImplementedError('action masks are a discrete-PPO feature')
+        self.has_central_value = config.get('central_value_config') is not None
+        if self.has_central_value:
+            raise NotImplementedError('central_value_config is served by rl_games_b200.agent_cv.A2CAgentCV: build the agent through '
+                                      'rl_games_b200.register(runner) / rl_games_b200.runner.continuous_agent, which pick it')
+        self.central_value_net = None
+        self.num_agents = self.env_info.get('agents', 1)
+        if self.num_agents != 1:
+            raise NotImplementedError('multi-agent envs are not on the B200 hot path yet')
+        if self.mask_autoreset_rows and self.num_agents > 1:
+            raise ValueError("PPO next_step autoreset masking does not support multi-agent envs; "
+                             "wrap the env with a same_step autoreset adapter instead")
+        self.schedule_type = config.get('schedule_type', 'per_minibatch')
+        if self.schedule_type == 'legacy':
+            self.schedule_type = 'per_minibatch'
+        if self.is_adaptive_lr and self.schedule_type not in ('per_minibatch', 'standard'):
+            raise NotImplementedError("adaptive lr_schedule with schedule_type=%r: 'per_minibatch' (the default) and 'standard' "
+                                      "(one step per mini-epoch) run on the device scheduler" % self.schedule_type)
+        # EMA advantage normaliser (a2c_common.py:369, :473-475): GeneralizedMovingStats((1,), decay=adv_rms_momentum), 'mean_std'
+        self.normalize_rms_advantage = bool(config.get('normalize_rms_advantage', False)) and self.normalize_advantage
+        self.adv_rms_momentum = float(config.get('adv_rms_momentum', 0.5))
+        if type(self.observation_space).__name__ == 'Dict':
+            raise NotImplementedError('Dict observation spaces are not on the B200 hot path yet')
+        self.obs_shape = self.observation_space.shape
+        if len(self.obs_shape) != 1:
+            raise NotImplementedError('only flat observations are on the B200 hot path')
+
+        # ---- ContinuousA2CBase (a2c_common.py:1484-1497) ----
+        self.is_discrete = False
+        action_space = self.env_info['action_space']
+        self.actions_num = action_space.shape[0]
+        self.bounds_loss_coef = config.get('bounds_loss_coef', None)
+        self.bound_loss_type = config.get('bound_loss_type', 'bound')
+        self.clip_actions = config.get('clip_actions', True)
+        self.actions_low = torch.from_numpy(np.asarray(action_space.low).copy()).float().to(self.device_t)
+        self.actions_high = torch.from_numpy(np.asarray(action_space.high).copy()).float().to(self.device_t)
+
+    # =============================================================================== allocation
     def init_tensors(self):
         """a2c_common.py:634-660 + experience.py:330-398: one time-major arena, zero-initialised."""
         if self._tensors_ready:
@@ -390,7 +246,7 @@ class A2CAgent(CompileTolerantModel):
             self.d_head = f(mb, A + 1)
         ops.set_pdl(self.config.get('b200_pdl', False))     # programmatic dependent launch: off by default
         if self.use_tc:
-            self.n_splits = 132      # split-partial rows: at least the fused backward kernels' grid (<= one CTA per SM)
+            self.n_splits = ops.NUM_SMS      # split-partial rows: at least the fused backward kernels' grid (<= one CTA per SM)
             tb = ops.tc_tile_bytes(m.D, m.units, A)
             nt = (mb + 127) // 128
             u8 = lambda n: torch.zeros(n, dtype=torch.uint8, device=dev)   # noqa: E731
@@ -437,7 +293,7 @@ class A2CAgent(CompileTolerantModel):
             self.t_hdense, self.t_hmlp, self.t_dHmlp = f(S, Hd), f(mb, Hd), f(mb, Hd)
             self.t_dgates, self.t_dhin, self.t_dcin = f(S, 4 * Hd), f(S, Hd), f(2, S, Hd)
         self.gae_partials = torch.zeros((N + 63) // 64, 8, dtype=torch.float64, device=dev)
-        self.loss_partials = torch.zeros(max((mb + 127) // 128, 132), ops.loss_partial_stride(), dtype=torch.float64, device=dev)
+        self.loss_partials = torch.zeros(max((mb + 127) // 128, ops.NUM_SMS), ops.loss_partial_stride(), dtype=torch.float64, device=dev)
         self.n_updates = self.mini_epochs_num * self.num_minibatches
         self.stats = f(self.n_updates, 16)
         # comm buffer = flat gradient + 1 KL slot (one all-reduce per minibatch, a2c_common.py:493-509 + :1559-1561)
@@ -476,7 +332,7 @@ class A2CAgent(CompileTolerantModel):
         if self.normalize_rms_advantage and not hasattr(self, 'adv_ema_state'):
             self.adv_ema_state = torch.zeros(2, dtype=torch.float32, device=dev)     # GeneralizedMovingStats: mean, mean of squares
             self.adv_ema_step = torch.ones(1, dtype=torch.int32, device=dev)
-        self.ra_nrm = torch.zeros(132, dtype=torch.float64, device=dev)      # reduce_adam: per-CTA sum-of-squares partials
+        self.ra_nrm = torch.zeros(ops.NUM_SMS, dtype=torch.float64, device=dev)      # reduce_adam: per-CTA sum-of-squares partials
         self.ra_bar = torch.zeros(1, dtype=torch.int64, device=dev)          # reduce_adam: monotonic grid-barrier counter
         self.host_stats = torch.zeros(self.n_updates, 16, dtype=torch.float32).pin_memory()
         self.host_state = torch.zeros(10, dtype=torch.float64).pin_memory()
@@ -578,11 +434,6 @@ class A2CAgent(CompileTolerantModel):
                                         float(self.gamma), int(bool(rs.log_val)), int(bool(self.value_bootstrap)))
         self._graph_update = None
         self._graph_epoch = None
-
-    def _meter_host(self):
-        if self._meter_cache is None:
-            self._meter_cache = self.meter.cpu().numpy()
-        return self._meter_cache
 
     # =============================================================================== env plumbing
     def cast_obs(self, obs, name='obs'):
@@ -1099,10 +950,6 @@ class A2CAgent(CompileTolerantModel):
     def set_train(self):
         self.model.train()
 
-    def update_epoch(self):
-        self.epoch_num += 1
-        return self.epoch_num
-
     def train_epoch(self, noise=None):
         """a2c_common.py:1517-1584.  Returns the reference tuple; the per-minibatch scalars are 0-dim views of
         one device stats block, read back with ONE D2H copy + sync per epoch."""
@@ -1201,153 +1048,19 @@ class A2CAgent(CompileTolerantModel):
     def _lr_dirty(self):
         return getattr(self, '_lr_synced', None) != self.last_lr
 
-    # =============================================================================== multi-GPU stats sync
-    def _stats_modules(self):
-        mods = []
-        if self.normalize_input:
-            mods.append(('obs', self.model.running_mean_std))
-        if self.normalize_value:
-            mods.append(('value', self.model.value_mean_std))
-        return mods
-
-    def sync_running_stats(self):
-        """a2c_common.py:782-808: pooled = all-reduce of per-epoch moment DELTAS (merge_rank_stats :61-93), packed into
-        one fp64 all-reduce for all normalisers; broadcast = rank 0's stats."""
-        if not self.multi_gpu or not self.multi_gpu_sync_stats:
-            return
-        mods = self._stats_modules()
-        if not mods:
-            return
-        if self.multi_gpu_sync_stats_mode == 'broadcast':
-            for _, m in mods:
-                for t in (m.count, m.running_mean, m.running_var):
-                    dist.broadcast(t, 0)
-                m.refresh()
-            return
-        self._stats_sync_obj().sync(lambda t: dist.all_reduce(t, op=dist.ReduceOp.SUM))
-        for _, m in mods:
-            m.refresh()
-
-    def _stats_sync_obj(self):
-        if getattr(self, '_stats_sync', None) is None:
-            self._stats_sync = PackedStatsSync([(n, m.count, m.running_mean, m.running_var) for n, m in self._stats_modules()])
-        return self._stats_sync
-
-    def _seed_stats_sync_snapshots(self):
-        """a2c_common.py:767-780"""
-        if not self.multi_gpu or not self.multi_gpu_sync_stats or self.multi_gpu_sync_stats_mode == 'broadcast':
-            return
-        self._stats_sync_obj().seed()
-
-    # =============================================================================== train loop
-    def train(self):
-        """a2c_common.py:1662-1782"""
-        self.init_tensors()
-        total_time = 0
-        self.obs = self.env_reset()
-        self.curr_frames = self.batch_size_envs
-        if self.multi_gpu:
-            dist.broadcast(self.model.flat, 0)      # replaces broadcast_object_list of the pickled state_dict (:1670-1680)
-            self._repack()
-        while True:
-            epoch_num = self.update_epoch()
-            step_time, play_time, update_time, sum_time, a_losses, c_losses, b_losses, entropies, kls, last_lr, lr_mul = self.train_epoch()
-            total_time += sum_time
-            curr_frames = self.curr_frames * self.world_size if self.multi_gpu else self.curr_frames
-            self.frame += curr_frames
-            frame = self.frame // self.num_agents
-            should_exit = False
-            if self.global_rank == 0:
-                if self.print_stats:
-                    st = max(step_time, 1e-9)
-                    print(f'fps step: {curr_frames / st:.0f} fps step and policy inference: {curr_frames / play_time:.0f} '
-                          f'fps total: {curr_frames / sum_time:.0f} epoch: {epoch_num:.0f}/{self.max_epochs:.0f} frames: {frame:.0f}')
-                self.write_stats(total_time, epoch_num, step_time, play_time, update_time, a_losses, c_losses, entropies, kls,
-                                 last_lr, lr_mul, frame, sum_time, play_time, curr_frames)
-                if self.bounds_loss_coef is not None:        # a2c_common.py:1705-1706 (after write_stats and the observer's scalars)
-                    self.writer.add_scalar('losses/bounds_loss', float(self.last_stats[:, 3].mean()), frame)
-                mean_rewards = None
-                if self.game_rewards.current_size > 0:
-                    mh = self._meter_host()
-                    # float32 array like AverageMeter.get_mean() (torch_ext.py:349-352): checkpoint names embed str() of it
-                    mean_rewards = np.asarray([mh[0]], dtype=np.float32)
-                    self.mean_rewards = mean_rewards[0]
-                    for tag, val in (('rewards', mh[0]), ('shaped_rewards', mh[1])):
-                        self.writer.add_scalar(tag + '/step', val, frame)
-                        self.writer.add_scalar(tag + '/iter', val, epoch_num)
-                        self.writer.add_scalar(tag + '/time', val, total_time)
-                    self.writer.add_scalar('episode_lengths/step', mh[2], frame)
-                    self.writer.add_scalar('episode_lengths/iter', mh[2], epoch_num)
-                    self.writer.add_scalar('episode_lengths/time', mh[2], total_time)
-                    checkpoint_name = self.config['name'] + '_ep_' + str(epoch_num) + '_rew_' + str(mean_rewards[0])
-                    if self.save_freq > 0 and epoch_num % self.save_freq == 0:
-                        self.save(os.path.join(self.nn_dir, 'last_' + checkpoint_name))
-                    if mean_rewards[0] > self.last_mean_rewards and epoch_num >= self.save_best_after:
-                        print('saving next best rewards: ', mean_rewards)
-                        self.last_mean_rewards = mean_rewards[0]
-                        self.save(os.path.join(self.nn_dir, self.config['name']))
-                        if 'score_to_win' in self.config and self.last_mean_rewards > self.config['score_to_win']:
-                            print('Maximum reward achieved. Network won!')
-                            self.save(os.path.join(self.nn_dir, checkpoint_name))
-                            should_exit = True
-                if epoch_num >= self.max_epochs and self.max_epochs != -1:
-                    if self.game_rewards.current_size == 0:
-                        print('WARNING: Max epochs reached before any env terminated at least once')
-                        mean_rewards = -np.inf
-                    self.save(os.path.join(self.nn_dir, 'last_' + self.config['name'] + '_ep_' + str(epoch_num)
-                                           + '_rew_' + str(mean_rewards).replace('[', '_').replace(']', '_')))
-                    print('MAX EPOCHS NUM!')
-                    should_exit = True
-                if self.frame >= self.max_frames and self.max_frames != -1:
-                    if self.game_rewards.current_size == 0:
-                        mean_rewards = -np.inf
-                    self.save(os.path.join(self.nn_dir, 'last_' + self.config['name'] + '_frame_' + str(self.frame)
-                                           + '_rew_' + str(mean_rewards).replace('[', '_').replace(']', '_')))
-                    print('MAX FRAMES NUM!')
-                    should_exit = True
-                if not should_exit and self.stop_fn is not None and self.stop_fn(self):
-                    self.save(os.path.join(self.nn_dir, 'last_' + self.config['name'] + '_custom_stop_ep_' + str(epoch_num)))
-                    print('Custom stop callback returned True. Stopping training.')
-                    should_exit = True
-            if self.multi_gpu:
-                t = torch.tensor(float(should_exit), device=self.device_t)
-                dist.broadcast(t, 0)
-                should_exit = bool(t.item())
-            if should_exit:
-                return self.last_mean_rewards, epoch_num
-
+    # =============================================================================== summaries
     def write_stats(self, total_time, epoch_num, step_time, play_time, update_time, a_losses, c_losses, entropies, kls,
                     last_lr, lr_mul, frame, scaled_time, scaled_play_time, curr_frames):
-        """a2c_common.py:527-547"""
-        w = self.writer
-        w.add_scalar('performance/step_inference_rl_update_fps', curr_frames / scaled_time, frame)
-        w.add_scalar('performance/step_inference_fps', curr_frames / scaled_play_time, frame)
-        w.add_scalar('performance/step_fps', curr_frames / max(step_time, 1e-9), frame)
-        w.add_scalar('performance/rl_update_time', update_time, frame)
-        w.add_scalar('performance/step_inference_time', play_time, frame)
-        w.add_scalar('performance/step_time', step_time, frame)
-        st = self.last_stats
-        w.add_scalar('losses/a_loss', float(st[:, 0].mean()), frame)
-        w.add_scalar('losses/c_loss', float(st[:, 1].mean()), frame)
-        w.add_scalar('losses/entropy', float(st[:, 2].mean()), frame)
-        w.add_scalar('info/last_lr', last_lr * lr_mul, frame)
-        w.add_scalar('info/lr_mul', lr_mul, frame)
-        w.add_scalar('info/e_clip', self.e_clip * lr_mul, frame)
-        w.add_scalar('info/kl', float(st[:, 4].mean()), frame)
-        w.add_scalar('info/epochs', epoch_num, frame)
-        self.algo_observer.after_print_stats(frame, epoch_num, total_time)
+        super().write_stats(total_time, epoch_num, step_time, play_time, update_time, a_losses, c_losses, entropies, kls,
+                            last_lr, lr_mul, frame, scaled_time, scaled_play_time, curr_frames)
+        if self.bounds_loss_coef is not None:        # a2c_common.py:1705-1706 (after write_stats and the observer's scalars)
+            self.writer.add_scalar('losses/bounds_loss', float(self.last_stats[:, 3].mean()), frame)
 
-    def clear_stats(self, clean_rewards=True):
-        self.meter.zero_()
-        self._meter_cache = None
-        if clean_rewards:
-            self.mean_rewards = self.last_mean_rewards = -float('inf')
-        self.algo_observer.after_clear_stats()
+    def _loss_means(self, a_losses, c_losses, entropies, kls):
+        st = self.last_stats
+        return float(st[:, 0].mean()), float(st[:, 1].mean()), float(st[:, 2].mean()), float(st[:, 4].mean())
 
     # =============================================================================== checkpoints (a2c_common.py:825-921)
-    def get_weights(self):
-        return {'model': self.model.state_dict()}
-
     def get_stats_weights(self, model_stats=False):
         state = {}
         if model_stats:
@@ -1364,7 +1077,7 @@ class A2CAgent(CompileTolerantModel):
             self.model.value_mean_std.load_state_dict(weights['reward_mean_std'])
 
     def set_weights(self, weights):
-        self.model.load_state_dict(weights['model'])
+        super().set_weights(weights)
         self.set_stats_weights(weights)
         self._seed_stats_sync_snapshots()
         self._repack()
@@ -1414,18 +1127,6 @@ class A2CAgent(CompileTolerantModel):
         if 'capability_manifest' in weights and self.config.get('capability_manifest') is None:
             self.config['capability_manifest'] = weights['capability_manifest']
         self._seed_stats_sync_snapshots()
-
-    def save(self, fn):
-        """torch_ext.save_checkpoint (torch_ext.py:90-92): `<fn>.pth` via torch.save"""
-        state = self.get_full_state_weights()
-        torch.save(state, fn + '.pth')
-
-    def restore(self, fn, set_epoch=True):
-        """torch_ext.load_checkpoint (torch_ext.py:94-112): strips `_orig_mod.` prefixes"""
-        checkpoint = torch.load(fn, map_location=self.device_t, weights_only=False)
-        if 'model' in checkpoint:
-            checkpoint['model'] = {k.replace('_orig_mod.', ''): v for k, v in checkpoint['model'].items()}
-        self.set_full_state_weights(checkpoint, set_epoch=set_epoch)
 
     def restore_central_value_function(self, fn):
         # the reference's Runner refuses this before it gets here (torch_runner.py:45-46)

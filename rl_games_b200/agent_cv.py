@@ -24,11 +24,13 @@ import torch.distributed as dist
 from . import ops
 from .agent import A2CAgent
 from .common import IdentityScheduler, LinearScheduler
-from .model import _RunningStats, check_network_params
+from .model import FlatParamModel, _RunningStats, check_network_params
 
 
-class CentralValueNet:
+class CentralValueNet(FlatParamModel):
     """CentralValueTrain on the fp32 kernels: flat arena [W0 b0 ... W_v b_v] in the reference's parameter order."""
+
+    ADAM_GROUP_EXTRA = {}          # central_value.py's Adam state dict: lr / betas / eps / weight_decay / params only
 
     # `CentralValueTrain.model` (central_value.py:44): the reference's Runner wraps it with torch.compile unless the YAML says
     # `torch_compile: False` (torch_runner.py:308-313).  Here the net IS its model and there is no nn.Module to compile: reading `.model`
@@ -85,18 +87,9 @@ class CentralValueNet:
             ins = u
         self.Hl = ins
         sizes += [('W_v', (1, ins)), ('b_v', (1,))]
-        self.layout, off = OrderedDict(), 0
-        for n, shp in sizes:
-            self.layout[n] = (off, shp)
-            off += int(torch.Size(shp).numel())
-        self.num_params = off
-        dev = self.device
-        self.flat = torch.zeros(off, dtype=torch.float32, device=dev)
-        self.exp_avg, self.exp_avg_sq = torch.zeros_like(self.flat), torch.zeros_like(self.flat)
-        for n, (o, shp) in self.layout.items():
-            if n.startswith('W'):
-                bound = 1.0 / float(shp[1]) ** 0.5
-                self.view(n).uniform_(-bound, bound)
+        self._init_arena(sizes)
+        off, dev = self.num_params, self.device
+        self._init_linear_default()
         self.running_mean_std = _RunningStats(self.S, dev) if self.normalize_input else None
         self.value_mean_std = _RunningStats(1, dev) if self.normalize_value else None
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)   # noqa: E731
@@ -111,7 +104,7 @@ class CentralValueNet:
         self.grad = f(off)
         self.loss_partials = torch.zeros((mb + 255) // 256, 8, dtype=torch.float64, device=dev)
         self.inv_counts = f(self.num_minibatches)
-        self.mom_scratch = torch.zeros(132 * 4 * 2 * self.S, dtype=torch.float64, device=dev)
+        self.mom_scratch = torch.zeros(ops.NUM_SMS * 4 * 2 * self.S, dtype=torch.float64, device=dev)
         self.counters = torch.zeros(4, dtype=torch.int32, device=dev)
         self.opt_state = torch.tensor([self.lr, 0.0, 0.0, 0.0], dtype=torch.float64, device=dev)
         self.adam_stats = f(16)
@@ -119,11 +112,6 @@ class CentralValueNet:
         self.opt_cfg = ops.OptCfg(0.9, 0.999, 1e-8, self.weight_decay, self.grad_norm, 0.0, 1e-6, 1e-2, 1.5,
                                   1.0 / (self.world_size if self.multi_gpu else 1), int(self.truncate_grads), 0)
         self.last_losses = []
-
-    def view(self, name, arena=None):
-        o, shp = self.layout[name]
-        a = self.flat if arena is None else arena
-        return a[o:o + int(torch.Size(shp).numel())].view(shp)
 
     def param_names(self):
         names = []
@@ -137,31 +125,10 @@ class CentralValueNet:
             out += [self.view(f'W{i}', arena), self.view(f'b{i}', arena)]
         return out + [self.view('W_v', arena), self.view('b_v', arena)]
 
-    def state_dict(self):
-        sd = OrderedDict()
-        if self.normalize_value:
-            sd.update(self.value_mean_std.state_dict('value_mean_std.'))
-        if self.normalize_input:
-            sd.update(self.running_mean_std.state_dict('running_mean_std.'))
-        for n, v in zip(self.param_names(), self._param_views()):
-            sd[n] = v.clone()
-        return sd
-
     def load_state_dict(self, sd, strict=True):
-        def strip(k):          # CentralValueTrain.state_dict() prefixes its model's keys with 'model.'; torch.compile adds '_orig_mod.'
-            k = k.replace('_orig_mod.', '')
-            return k[len('model.'):] if k.startswith('model.') else k
-        sd = {strip(k): v for k, v in sd.items()}
-        with torch.no_grad():
-            for n, v in zip(self.param_names(), self._param_views()):
-                if n in sd:
-                    v.copy_(sd[n].reshape(v.shape))
-                elif strict:
-                    raise KeyError(f'missing key in central value state_dict: {n}')
-            if self.normalize_value and 'value_mean_std.running_mean' in sd:
-                self.value_mean_std.load_state_dict(sd, 'value_mean_std.')
-            if self.normalize_input and 'running_mean_std.running_mean' in sd:
-                self.running_mean_std.load_state_dict(sd, 'running_mean_std.')
+        # CentralValueTrain.state_dict() prefixes its model's keys with 'model.'; torch.compile adds '_orig_mod.'
+        sd = {k.replace('_orig_mod.', ''): v for k, v in sd.items()}
+        super().load_state_dict({k[len('model.'):] if k.startswith('model.') else k: v for k, v in sd.items()}, strict)
 
     # ---------------------------------------------------------------------------------------------- forward
     def _trunk(self, x, acts, M, rows_per_chunk=None, chunk_stride=0):
@@ -316,10 +283,7 @@ class A2CAgentCV(A2CAgent):
         state = super().get_full_state_weights()
         cv = self.central_value_net
         state['assymetric_vf_nets'] = OrderedDict(('model.' + k, v) for k, v in cv.state_dict().items())
-        st = {i: {'step': torch.tensor(float(cv.opt_state.cpu()[1])), 'exp_avg': m.clone(), 'exp_avg_sq': v.clone()}
-              for i, (m, v) in enumerate(zip(cv._param_views(cv.exp_avg), cv._param_views(cv.exp_avg_sq)))}
-        state['assymetric_vf_optimizer'] = {'state': st, 'param_groups': [{'lr': cv.lr, 'betas': (0.9, 0.999), 'eps': 1e-08,
-                                                                          'weight_decay': cv.weight_decay, 'params': list(range(len(st)))}]}
+        state['assymetric_vf_optimizer'] = cv.optimizer_state_dict(cv.lr, float(cv.opt_state.cpu()[1]), cv.weight_decay)
         return state
 
     def restore_central_value_function(self, fn):
@@ -339,12 +303,7 @@ class A2CAgentCV(A2CAgent):
             cv.load_state_dict(weights['assymetric_vf_nets'])
         osd = weights.get('assymetric_vf_optimizer')
         if osd:
-            step = 0
-            for i, (m, v) in enumerate(zip(cv._param_views(cv.exp_avg), cv._param_views(cv.exp_avg_sq))):
-                if i in osd['state']:
-                    m.copy_(osd['state'][i]['exp_avg'].reshape(m.shape))
-                    v.copy_(osd['state'][i]['exp_avg_sq'].reshape(v.shape))
-                    step = int(float(osd['state'][i]['step']))
-            cv.lr = float(osd['param_groups'][0]['lr'])
+            lr, step = cv.load_optimizer_state_dict(osd)
+            cv.lr = float(lr)
             cv.opt_state.copy_(torch.tensor([cv.lr, float(step), 0.9 ** step if step else 0.0, 0.999 ** step if step else 0.0],
                                             dtype=torch.float64))

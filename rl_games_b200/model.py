@@ -14,6 +14,10 @@ arenas, so the optimiser, the gradient all-reduce and the checkpoint code each t
 (``a2c_network.sigma``, ``a2c_network.actor_mlp.{0,2,..}.{weight,bias}``, ``a2c_network.value.*``,
 ``a2c_network.mu.*``, ``running_mean_std.*``, ``value_mean_std.*``) so checkpoints interoperate with the
 reference trainer and players.
+
+``FlatParamModel`` owns what every flat-arena network shares -- the layout, ``view()``, the state dicts and the torch Adam state
+dict -- for ``B200Model`` and for the discrete model (agent_discrete.py) and the central value net (agent_cv.py), which only define
+their layouts and key names.
 """
 import math
 from collections import OrderedDict
@@ -156,11 +160,90 @@ def _model_call(self, *args, **kwargs):
                               'it has no module-style forward')
 
 
-class B200Model:
+class FlatParamModel:
+    """All parameters of a network in ONE flat fp32 arena (``flat``) with matching Adam-moment arenas (``exp_avg``, ``exp_avg_sq``),
+    laid out from an ordered ``(name, shape)`` list.  Subclasses define ``param_names()`` and ``_param_views(arena)``: the reference's
+    state-dict keys and the matching views, in the reference's ``model.parameters()`` order, which is also the index order of the
+    torch Adam state.  They also set ``device``, ``normalize_input`` / ``normalize_value`` and ``running_mean_std`` /
+    ``value_mean_std``."""
+
     __call__ = _model_call
 
-    RNN_KEYS = (('a2c_network.rnn.rnn.weight_ih_l0', 'W_ih'), ('a2c_network.rnn.rnn.weight_hh_l0', 'W_hh'),
-                ('a2c_network.rnn.rnn.bias_ih_l0', 'b_ih'), ('a2c_network.rnn.rnn.bias_hh_l0', 'b_hh'))
+    # torch.optim.Adam param-group keys written after lr / betas / eps / weight_decay
+    ADAM_GROUP_EXTRA = {'amsgrad': False, 'maximize': False, 'foreach': None, 'capturable': False, 'differentiable': False, 'fused': True,
+                        'decoupled_weight_decay': False}
+
+    def _init_arena(self, sizes, align=1):
+        """layout[name] = (offset, shape); every tensor starts on a multiple of `align` elements"""
+        self.layout, off = OrderedDict(), 0
+        for n, shp in sizes:
+            off = (off + align - 1) // align * align
+            self.layout[n] = (off, shp)
+            off += int(torch.Size(shp).numel())
+        self.num_params = off
+        self.flat = torch.zeros(off, dtype=torch.float32, device=self.device)
+        self.exp_avg = torch.zeros_like(self.flat)
+        self.exp_avg_sq = torch.zeros_like(self.flat)
+
+    def _init_linear_default(self):
+        """torch.nn.Linear default weights (U(-1/sqrt(fan_in), 1/sqrt(fan_in)), drawn in layout order), zero biases"""
+        for n, (o, shp) in self.layout.items():
+            if n.startswith('W'):
+                bound = 1.0 / float(shp[1]) ** 0.5
+                self.view(n).uniform_(-bound, bound)
+
+    def view(self, name, arena=None):
+        off, shp = self.layout[name]
+        arena = self.flat if arena is None else arena
+        return arena[off:off + int(torch.Size(shp).numel())].view(shp)
+
+    def state_dict(self):
+        sd = OrderedDict()
+        if self.normalize_value:
+            sd.update(self.value_mean_std.state_dict('value_mean_std.'))
+        if self.normalize_input:
+            sd.update(self.running_mean_std.state_dict('running_mean_std.'))
+        for n, v in zip(self.param_names(), self._param_views()):
+            sd[n] = v.clone()
+        return sd
+
+    def load_state_dict(self, sd, strict=True):
+        sd = {k.replace('_orig_mod.', ''): v for k, v in sd.items()}
+        missing = [n for n in self.param_names() if n not in sd]
+        if missing and strict:
+            raise KeyError(f'missing keys in state_dict: {missing}')
+        with torch.no_grad():
+            for n, v in zip(self.param_names(), self._param_views()):
+                if n in sd:
+                    v.copy_(sd[n].reshape(v.shape))
+            if self.normalize_value and 'value_mean_std.running_mean' in sd:
+                self.value_mean_std.load_state_dict(sd, 'value_mean_std.')
+            if self.normalize_input and 'running_mean_std.running_mean' in sd:
+                self.running_mean_std.load_state_dict(sd, 'running_mean_std.')
+
+    def optimizer_state_dict(self, lr, step, weight_decay):
+        """torch.optim.Adam.state_dict() layout (index-keyed, reference parameter order)."""
+        state = {i: {'step': torch.tensor(float(step)), 'exp_avg': m.clone(), 'exp_avg_sq': v.clone()}
+                 for i, (m, v) in enumerate(zip(self._param_views(self.exp_avg), self._param_views(self.exp_avg_sq)))}
+        group = {'lr': lr, 'betas': (0.9, 0.999), 'eps': 1e-08, 'weight_decay': weight_decay, **self.ADAM_GROUP_EXTRA,
+                 'params': list(range(len(state)))}
+        return {'state': state, 'param_groups': [group]}
+
+    def load_optimizer_state_dict(self, osd):
+        """Returns (lr, step); lr is None when the dict has no param group."""
+        st, step = osd.get('state', {}), 0
+        ms, vs = self._param_views(self.exp_avg), self._param_views(self.exp_avg_sq)
+        for i in range(len(ms)):
+            if i in st:
+                ms[i].copy_(st[i]['exp_avg'].reshape(ms[i].shape))
+                vs[i].copy_(st[i]['exp_avg_sq'].reshape(vs[i].shape))
+                step = int(float(st[i]['step']))
+        return (osd['param_groups'][0]['lr'] if osd.get('param_groups') else None), step
+
+
+class B200Model(FlatParamModel):
+    RNN_KEYS = ('a2c_network.rnn.rnn.weight_ih_l0', 'a2c_network.rnn.rnn.weight_hh_l0', 'a2c_network.rnn.rnn.bias_ih_l0',
+                'a2c_network.rnn.rnn.bias_hh_l0')
 
     def __init__(self, network_params, obs_dim, act_dim, device, normalize_input, normalize_value, value_size=1,
                  seed=None):
@@ -229,22 +312,13 @@ class B200Model:
             ins = Hd                     # the heads read the LSTM output
         self.Hl = ins
         sizes += [('W_head', (self.A + 1, ins)), ('b_head', (self.A + 1,))]
-        self.layout = OrderedDict()
-        off = 0
-        for n, shp in sizes:
-            numel = int(torch.Size(shp).numel())
-            # every tensor starts on an 8-element boundary (32 bytes in the fp32 arenas, 16 bytes in the bf16 twin the tensor-core GEMMs
-            # read): weight rows can then be staged with 16-byte loads whatever the action count did to the offsets.  The gaps hold
-            # zeros in every arena (weights, gradients, moments), so norms, Adam and the all-reduce are unaffected; layouts whose tensor
-            # sizes are all multiples of 8 (the BASELINE MLPs with 8 actions) have no gaps at all.
-            off = (off + 7) // 8 * 8
-            self.layout[n] = (off, shp)
-            off += numel
-        self.num_params = off
-        self.flat = torch.zeros(off, dtype=torch.float32, device=self.device)
+        # every tensor starts on an 8-element boundary (32 bytes in the fp32 arenas, 16 bytes in the bf16 twin the tensor-core GEMMs
+        # read): weight rows can then be staged with 16-byte loads whatever the action count did to the offsets.  The gaps hold
+        # zeros in every arena (weights, gradients, moments), so norms, Adam and the all-reduce are unaffected; layouts whose tensor
+        # sizes are all multiples of 8 (the BASELINE MLPs with 8 actions) have no gaps at all.
+        self._init_arena(sizes, align=8)
+        off = self.num_params
         self.grad = torch.zeros(off, dtype=torch.float32, device=self.device)
-        self.exp_avg = torch.zeros(off, dtype=torch.float32, device=self.device)
-        self.exp_avg_sq = torch.zeros(off, dtype=torch.float32, device=self.device)
         self.W = [self.view(f'W{i}') for i in range(len(self.units))]
         self.b = [self.view(f'b{i}') for i in range(len(self.units))]
         self.sigma = self.view('sigma')
@@ -289,11 +363,6 @@ class B200Model:
             torch.add(self.sigma_chain, self.min_sigma, out=self.logstd_eff)
             self.sigma_chain.div_(self.logstd_eff)
             self.logstd_eff.log_()
-
-    def view(self, name, arena=None):
-        off, shp = self.layout[name]
-        arena = self.flat if arena is None else arena
-        return arena[off:off + int(torch.Size(shp).numel())].view(shp)
 
     def _init_weights(self, network_params, seed):
         """network_builder.py:326-348: mlp initializer on every Linear weight, zero biases, mu_init on mu.weight,
@@ -363,7 +432,7 @@ class B200Model:
         """Reference parameter order (optimizer state is index-keyed): sigma, actor_mlp.*, value.*, mu.*"""
         return self._param_views(self.flat)
 
-    def _param_views(self, arena):
+    def _param_views(self, arena=None):
         if self.separate:
             return self._param_views_separate(arena)
         out = [self.view('sigma', arena)]
@@ -390,89 +459,20 @@ class B200Model:
         out += [wh[:1, tu[-1]:], bh[:1], wh[1:, :tu[-1]], bh[1:]]
         return out
 
-    def _separate_keys(self):
+    def param_names(self):
+        """state-dict keys of _param_views, in the same order: sigma, actor_mlp.*, [critic_mlp.*], [rnn.*], value.*, mu.*"""
         keys = ['a2c_network.sigma']
-        for trunk in ('actor_mlp', 'critic_mlp'):
+        for trunk in (('actor_mlp', 'critic_mlp') if self.separate else ('actor_mlp',)):
             for i in range(len(self.trunk_units)):
                 keys += [f'a2c_network.{trunk}.{2 * i}.weight', f'a2c_network.{trunk}.{2 * i}.bias']
+        if self.rnn_units:
+            keys += list(self.RNN_KEYS)
         return keys + ['a2c_network.value.weight', 'a2c_network.value.bias', 'a2c_network.mu.weight', 'a2c_network.mu.bias']
 
-    def state_dict(self):
-        sd = OrderedDict()
-        if self.normalize_value:
-            sd.update(self.value_mean_std.state_dict('value_mean_std.'))
-        if self.normalize_input:
-            sd.update(self.running_mean_std.state_dict('running_mean_std.'))
-        if self.separate:
-            for k, v in zip(self._separate_keys(), self._param_views(self.flat)):
-                sd[k] = v.clone()
-            return sd
-        sd['a2c_network.sigma'] = self.sigma.clone()
-        for i in range(len(self.units)):
-            sd[f'a2c_network.actor_mlp.{2 * i}.weight'] = self.W[i].clone()
-            sd[f'a2c_network.actor_mlp.{2 * i}.bias'] = self.b[i].clone()
-        for key, n in self.RNN_KEYS:
-            if self.rnn_units:
-                sd[key] = self.view(n).clone()
-        sd['a2c_network.value.weight'] = self.W_head[:1].clone()
-        sd['a2c_network.value.bias'] = self.b_head[:1].clone()
-        sd['a2c_network.mu.weight'] = self.W_head[1:].clone()
-        sd['a2c_network.mu.bias'] = self.b_head[1:].clone()
-        return sd
-
     def load_state_dict(self, sd, strict=True):
+        """strict: the normaliser statistics are required as well"""
         sd = {k.replace('_orig_mod.', ''): v for k, v in sd.items()}
-        need = [k for k in self.state_dict().keys()]
-        missing = [k for k in need if k not in sd]
+        missing = [k for k in self.state_dict() if k not in sd]
         if missing and strict:
             raise KeyError(f'missing keys in state_dict: {missing}')
-        with torch.no_grad():
-            if self.separate:
-                for k, v in zip(self._separate_keys(), self._param_views(self.flat)):
-                    if k in sd:
-                        v.copy_(sd[k].reshape(v.shape))
-                self._load_normalisers(sd)
-                return
-            if 'a2c_network.sigma' in sd:
-                self.sigma.copy_(sd['a2c_network.sigma'])
-            for i in range(len(self.units)):
-                self.W[i].copy_(sd[f'a2c_network.actor_mlp.{2 * i}.weight'])
-                self.b[i].copy_(sd[f'a2c_network.actor_mlp.{2 * i}.bias'])
-            if self.rnn_units:
-                for key, n in self.RNN_KEYS:
-                    self.view(n).copy_(sd[key])
-            self.W_head[:1].copy_(sd['a2c_network.value.weight'])
-            self.b_head[:1].copy_(sd['a2c_network.value.bias'])
-            self.W_head[1:].copy_(sd['a2c_network.mu.weight'])
-            self.b_head[1:].copy_(sd['a2c_network.mu.bias'])
-            self._load_normalisers(sd)
-
-    def _load_normalisers(self, sd):
-        if self.normalize_value and 'value_mean_std.running_mean' in sd:
-            self.value_mean_std.load_state_dict(sd, 'value_mean_std.')
-        if self.normalize_input and 'running_mean_std.running_mean' in sd:
-            self.running_mean_std.load_state_dict(sd, 'running_mean_std.')
-
-    # ------------------------------------------------------------------------------------------- optimizer state
-    def optimizer_state_dict(self, lr, step, weight_decay):
-        """torch.optim.Adam.state_dict() layout (index-keyed, reference parameter order)."""
-        state = {}
-        for i, (m, v) in enumerate(zip(self._param_views(self.exp_avg), self._param_views(self.exp_avg_sq))):
-            state[i] = {'step': torch.tensor(float(step)), 'exp_avg': m.clone(), 'exp_avg_sq': v.clone()}
-        group = {'lr': lr, 'betas': (0.9, 0.999), 'eps': 1e-08, 'weight_decay': weight_decay, 'amsgrad': False,
-                 'maximize': False, 'foreach': None, 'capturable': False, 'differentiable': False, 'fused': True,
-                 'decoupled_weight_decay': False, 'params': list(range(len(state)))}
-        return {'state': state, 'param_groups': [group]}
-
-    def load_optimizer_state_dict(self, osd):
-        """Returns (lr, step)."""
-        st = osd.get('state', {})
-        step = 0
-        ms, vs = self._param_views(self.exp_avg), self._param_views(self.exp_avg_sq)
-        for i in range(len(ms)):
-            if i in st:
-                ms[i].copy_(st[i]['exp_avg'].reshape(ms[i].shape))
-                vs[i].copy_(st[i]['exp_avg_sq'].reshape(vs[i].shape))
-                step = int(float(st[i]['step']))
-        lr = osd['param_groups'][0]['lr'] if osd.get('param_groups') else None
-        return lr, step
+        super().load_state_dict(sd, strict=False)

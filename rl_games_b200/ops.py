@@ -10,6 +10,8 @@ import torch
 from ._lib import lib, check, ptr, B200RLError
 
 ACT = {'None': 0, None: 0, 'none': 0, 'elu': 1, 'relu': 2, 'tanh': 3}
+# streaming multiprocessors of the H100 SXM: sizes the host buffers that hold one row per CTA of a grid capped at one CTA per SM
+NUM_SMS = 132
 
 
 class LossCfg(ctypes.Structure):
