@@ -7,13 +7,14 @@
 //   bwd1          : delta chain d_head -> d3 -> d2 -> d1 (dgrad) + weight grads of the head and layer 3 + bias grads.
 //   bwd2          : weight grads of layers 2 and 1 (+ bias grad of layer 1).
 //
-// All GEMMs are M = 128-row wgmma chains run by every warpgroup of the CTA (tc::mma128: fp32 accumulators in the per-CTA
-// accumulator buffer, addressed by lane = row and column like tensor memory, read back one row per thread); operands are
-// INTERLEAVE shared-memory tiles (tc_common.cuh).  One packed bf16 copy of each weight matrix serves the forward
+// All GEMMs are M = 128-row wgmma chains run by every warpgroup of the CTA.  The backward kernels (bwd1 / bwd2 bodies) keep their fp32
+// accumulators in the warpgroups' registers (tc::mma_frag); the forward, the layer-1 kernels and the pipelined bwd2 use tc::mma128 (fp32
+// accumulators in the per-CTA accumulator buffer, addressed by lane = row and column like tensor memory, read back one row per thread).
+// Operands are INTERLEAVE shared-memory tiles (tc_common.cuh).  One packed bf16 copy of each weight matrix serves the forward
 // (K-major view) and the dgrad (MN-major view); one copy of each activation / delta tile serves the dgrad
 // (K-major) and the wgrad (MN-major) MMAs -- no transposes anywhere.  Tiles move global<->shared with
-// cp.async.bulk (1-D TMA) + mbarrier transaction counts; weight gradients stay resident in the accumulator buffer across all tiles a
-// persistent CTA processes and are flushed once per CTA into a [n_cta][P] partial buffer that the deterministic
+// cp.async.bulk (1-D TMA) + mbarrier transaction counts; weight gradients stay resident (registers or accumulator buffer) across all
+// tiles a persistent CTA processes and are flushed once per CTA into a [n_cta][P] partial buffer that the deterministic
 // split reducer (mlp_simt.cu) sums.
 #define TC_ACC_POOL_CTAS 132       // tc_grid(): at most one persistent CTA per SM
 #include "common.cuh"
@@ -76,19 +77,13 @@ __device__ __forceinline__ void bias_act(float (&v)[NV], const float* __restrict
         for (int j = 0; j < NV; ++j) v[j] = v[j] + bias[j];
     }
 }
-// v[j] *= act'(.) expressed through the activation OUTPUT a[j] (8 bf16 values of one chunk)
-__device__ __forceinline__ void mul_act_grad8(float* v, const float (&a)[8]) {
+// v * act'(.) expressed through the activation OUTPUT a
+__device__ __forceinline__ float mul_act_grad(float v, float a) {
     constexpr int act = TC_ACT;
-    if (act == B200RL_ACT_ELU) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] *= elu_grad_from_out(a[j]);
-    } else if (act == B200RL_ACT_RELU) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = a[j] > 0.f ? v[j] : 0.f;
-    } else if (act == B200RL_ACT_TANH) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] *= 1.0f - a[j] * a[j];
-    }
+    if (act == B200RL_ACT_ELU) return v * elu_grad_from_out(a);
+    if (act == B200RL_ACT_RELU) return a > 0.f ? v : 0.f;
+    if (act == B200RL_ACT_TANH) return v * (1.0f - a * a);
+    return v;
 }
 __device__ __forceinline__ void unpack8_bf16(const uint4& u, float* f) {
     const __nv_bfloat162* p = reinterpret_cast<const __nv_bfloat162*>(&u);
@@ -275,14 +270,14 @@ __device__ __forceinline__ void stage_x_tile_smem(uint8_t* sX, const float* sRaw
 // (chunk (g, r) sits at g * CS + r * 16).  Thread (g, rs) = (tid / RS, tid % RS) adds rows rs, rs + RS, ... of its 8 columns
 // (a quarter-warp reads 8 consecutive 16 B chunks: conflict-free), the RS partials are combined with warp shuffles in a fixed
 // order, and the lane with rs == 0 accumulates the result into its 8 running sums.  Whole warps either take part or skip.
-template <int R, int G, uint32_t CS, int T>
+template <int R, int G, uint32_t CS, int T, int UNROLL = 4>
 __device__ __forceinline__ void colsum8(const uint8_t* sT, int tid, float (&acc)[8]) {
     constexpr int RS = (T / G) < 32 ? (T / G) : 32;
     static_assert((RS & (RS - 1)) == 0 && RS >= 1 && RS * G <= T && (RS * G) % 32 == 0, "colsum8 thread mapping");
     const int rs = tid % RS, g = tid / RS;
     if (g >= G) return;
     float s[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll 4
+#pragma unroll UNROLL
     for (int r = rs; r < R; r += RS) {
         float a[8];
         unpack8_bf16(*reinterpret_cast<const uint4*>(sT + g * CS + r * 16), a);
@@ -817,34 +812,92 @@ struct Bwd1Args {
     int u1, u2, u3, act;
 };
 
-// body: TMEM (512 columns at `tmem`) is allocated by the calling kernel; barriers and shared-memory layout are set up here
+// The fused backward kernels keep every accumulator in registers (tc::mma_frag): 4 warpgroups, warpgroup wg owns the rows
+// [64 (wg & 1), +64) and the column half (wg >> 1) of each 128-row delta layer, and one [64 x NS] block of each weight gradient,
+// which stays in its registers over all tiles of the persistent CTA and is written once, by the flush.
+constexpr int BWD_THREADS = 512;
+
+// byte offset of the bf16 pair (row r, columns c, c + 1), c even, in a 128-row activation / delta tile
+__device__ __forceinline__ uint32_t pair_off(int r, int c) { return (uint32_t)r * 16u + (uint32_t)(c & 7) * 2u + (uint32_t)(c >> 3) * 2048u; }
+
+// The activation outputs that belong to a [64 x NS] fragment whose d[0] sits at byte offset off0 (pair_off) of the tile aT: two bf16
+// pairs per 8 columns.  The 32 lanes of a warp read one 128-byte core matrix per access (tc_common.cuh): conflict-free in shared memory,
+// one full segment in global memory.
+template <int NS, bool GLOBAL>
+__device__ __forceinline__ void load_act_frag(uint32_t (&ua)[NS / 4], const uint8_t* aT, uint32_t off0) {
+#pragma unroll
+    for (int i = 0; i < NS / 4; ++i) {
+        const uint32_t* src = reinterpret_cast<const uint32_t*>(aT + off0 + (i >> 1) * 2048u + (i & 1) * 128u);
+        ua[i] = GLOBAL ? __ldg(src) : *src;
+    }
+}
+// delta = dpre * act'(a) on the fragment, rounded to bf16 pairs and stored at the fragment's own positions of the shared delta tile
+// (operand of the next MMAs) and / or the global one
+template <int NS>
+__device__ __forceinline__ void delta_epilogue(const float (&d)[NS / 2], const uint32_t (&ua)[NS / 4], uint8_t* sT, uint8_t* gT, uint32_t off0) {
+#pragma unroll
+    for (int i = 0; i < NS / 4; ++i) {
+        const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&ua[i]));
+        const __nv_bfloat162 o = __floats2bfloat162_rn(mul_act_grad(d[2 * i], a.x), mul_act_grad(d[2 * i + 1], a.y));
+        const uint32_t off = off0 + (i >> 1) * 2048u + (i & 1) * 128u;
+        if (sT) *reinterpret_cast<uint32_t*>(sT + off) = *reinterpret_cast<const uint32_t*>(&o);
+        if (gT) *reinterpret_cast<uint32_t*>(gT + off) = *reinterpret_cast<const uint32_t*>(&o);
+    }
+}
+// one tile's column sums added to the running bias-gradient sums in shared memory (each sum has one owning thread).  colsum8 keeps its
+// 256-thread mapping whatever the CTA size is, so the order of the additions is fixed; the upper warpgroups skip it.  UNROLL = loads in
+// flight per thread (phase 2 runs it beside 96 live accumulator registers).
+template <int G, int UNROLL = 4>
+__device__ __forceinline__ void bias_colsum(const uint8_t* sT, int tid, float* sSum) {
+    float s[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    colsum8<128, G, 2048u, 256, UNROLL>(sT, tid, s);
+    const int g = colsum8_owner_group<G, 256>(tid);
+    if (g >= 0) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) sSum[g * 8 + j] += s[j];
+    }
+}
+__device__ __forceinline__ void flush_bias(const float* sSum, int n, float* dst, int tid) {
+    if (tid < n) dst[tid] = sSum[tid];
+}
+// a [64 x NS] fragment of a transposed weight gradient into the split-gradient row: element (in index i, out index o) ->
+// dst[o * ld + i] for i < ni, o < no; i0 / o0 = indices of d[0].  A warp writes 4 runs of 8 consecutive floats per store.
+template <int NS>
+__device__ __forceinline__ void flush_frag(const float (&d)[NS / 2], float* dst, int ld, int i0, int o0, int ni, int no) {
+#pragma unroll
+    for (int j = 0; j < NS / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int i = i0 + (e >> 1) * 8, o = o0 + 8 * j + (e & 1);
+            if (i < ni && o < no) dst[o * ld + i] = d[4 * j + e];
+        }
+    }
+}
+
+// body: barriers and shared-memory layout are set up here
 template <class N>
-__device__ __forceinline__ void bwd1_body(const Bwd1Args& p, uint8_t* smem, const uint32_t tmem) {
+__device__ __forceinline__ void bwd1_body(const Bwd1Args& p, uint8_t* smem) {
     uint8_t* sWh = smem; uint8_t* sW3 = sWh + N::WH_BYTES; uint8_t* sW2 = sW3 + N::W3_BYTES;
     uint8_t* sDH = sW2 + N::W2_BYTES;
-    uint8_t* sA3 = sDH + N::DH_BYTES;             // padded to 128 columns (upper col-groups stay zero)
-    uint8_t* sA2 = sA3 + 128 * 256;
+    uint8_t* sA3 = sDH + N::DH_BYTES;
+    uint8_t* sA2 = sA3 + N::A3_BYTES;
     uint8_t* sD3 = sA2 + N::A2_BYTES;
     uint8_t* sD2 = sD3 + N::A3_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sD2 + N::A2_BYTES);       // [0] weights, [1] tile loads, [2..4] mma
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int q = warp & 3, h = warp >> 2;
-    const int row = q * 32 + lane;
+    float* sBh = reinterpret_cast<float*>(sD2 + N::A2_BYTES); float* sB3 = sBh + N::AP; float* sB2 = sB3 + N::U3;   // running bias-gradient sums
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sB2 + N::U2);       // [0] weights, [1] tile loads
+    const int tid = threadIdx.x, wg = tid >> 7;
+    const int mh = wg & 1, nh = wg >> 1;
     const int n_tiles = (p.M + 127) / 128;
     int n_stamp = 0; (void)n_stamp;
     constexpr int TSB = 128; (void)TSB;
     TSTAMP();   // kernel start
     if (tid == 0) {
-        for (int i = 0; i < 5; ++i) mbar_init(&bars[i], 1);
+        mbar_init(&bars[0], 1); mbar_init(&bars[1], 1);
         fence_mbar_init();
     }
-    // zero the padding col-groups of the a3 tile once
-    for (int i = tid; i < (128 * 256 - (int)N::A3_BYTES) / 16; i += 256) reinterpret_cast<uint4*>(sA3 + N::A3_BYTES)[i] = make_uint4(0, 0, 0, 0);
-    fence_async_smem();
+    for (int i = tid; i < N::AP + N::U3 + N::U2; i += BWD_THREADS) sBh[i] = 0.f;
     __syncthreads();
     pdl_sync();      // everything above is CTA-local; all global traffic comes after the predecessor (the forward kernel) completed
-    const uint32_t TT = tmem, TWH = tmem + 256, TW3 = tmem + 288;     // transient [0,256), dWh^T [256,272), dW3^T [288,352)
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
     if (tid == 0) {
         mbar_expect_tx(&bars[0], N::WH_BYTES + N::W3_BYTES + N::W2_BYTES);
         bulk_g2s(sWh, p.wpack + N::WH_OFF, N::WH_BYTES, &bars[0]);
@@ -858,8 +911,20 @@ __device__ __forceinline__ void bwd1_body(const Bwd1Args& p, uint8_t* smem, cons
             bulk_g2s(sA2, p.act2 + (size_t)tile * N::A2_BYTES, N::A2_BYTES, &bars[1]);
         }
     }
-    // running bias-gradient sums: 8 columns per owning thread (colsum8)
-    float bsum3[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, bsum2[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, bsumh[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    // operand views (tc_common.cuh): K-major rows advance by ARS per 8, MN-major columns by the column-group stride per 8
+    constexpr uint32_t ACS = N::ACS, ARS = N::ARS;
+    const uint32_t uWh = smem_u32(sWh), uW3 = smem_u32(sW3), uW2 = smem_u32(sW2), uDH = smem_u32(sDH), uA3 = smem_u32(sA3), uA2 = smem_u32(sA2),
+                   uD3 = smem_u32(sD3), uD2 = smem_u32(sD2);
+    // fragment positions of this thread in the delta tiles: d3 [64 x 32], d2 [64 x 64], d1 two [64 x 64] halves
+    const int fr = 64 * mh + frag_row(), fc = frag_col();
+    const uint32_t off3 = pair_off(fr, 32 * nh + fc), off2 = pair_off(fr, 64 * nh + fc), off1 = pair_off(fr, 128 * nh + fc);
+    // weight gradients resident over all tiles: dWh^T [U3 x AP] in warpgroup 0, dW3^T [U2 x U3] as [64 x 32] blocks (mh, nh)
+    static_assert(N::U3 == 64 && N::U2 == 128 && N::U1 == 256, "fragment split of the backward kernel");
+    float dWh[N::AP / 2], dW3[16];
+#pragma unroll
+    for (int j = 0; j < N::AP / 2; ++j) dWh[j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) dW3[j] = 0.f;
     uint32_t phase = 0;
     bool first = true;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -867,163 +932,86 @@ __device__ __forceinline__ void bwd1_body(const Bwd1Args& p, uint8_t* smem, cons
         TSTAMP();   // tile start
         mbar_wait(&bars[1], phase);
         TSTAMP();   // tile loads landed
-        // ---- d3pre = d_head . Wh   ;  dWh^T += a3^T . d_head ----
-        mma128<N::U3, 0, 1, 2>(TT, 1, false, [&](int k, uint64_t& a, uint64_t& b) {
-            a = make_smem_desc(smem_u32(sDH) + k * 2 * N::ACS, N::ACS, N::ARS);
-            b = make_smem_desc(smem_u32(sWh), 128, N::WH_CS);
-        });
-        mma128<N::AP, 1, 1, 2>(TWH, 8, !first, [&](int k, uint64_t& a, uint64_t& b) {
-            a = make_smem_desc(smem_u32(sA3) + k * 256, 128, N::ACS);
-            b = make_smem_desc(smem_u32(sDH) + k * 256, 128, N::ACS);
-        });
-        colsum8<128, N::AP / 8, N::ACS, 256>(sDH, tid, bsumh);     // bias grad of the heads
-        TSTAMP();   // MMA a done
-        {   // d3 = d3pre * elu'(a3): U3/2 = 32 columns per thread
-            const int c0 = h * (N::U3 / 2);
-            float v[32];
-            tmem_ld32(TT + lane_base + c0, v);
+        {   // ---- d3pre = d_head . Wh   ;  dWh^T += a3^T . d_head ----
+            float d[16];
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                float a[8];
-                unpack8_bf16(*reinterpret_cast<const uint4*>(sA3 + tile_off(row, c0 / 8 + g, N::ACS, N::ARS)), a);
-                mul_act_grad8(&v[g * 8], a);
-            }
-            store_chunks32(v, row, c0, sD3, nullptr);
+            for (int j = 0; j < 16; ++j) d[j] = 0.f;
+            mma_frag<32, 0, 1, 1>(d, MmaOperand{uDH + mh * 8 * ARS, 2 * ACS, ACS, ARS}, MmaOperand{uWh + nh * 4 * N::WH_CS, 256, 128, N::WH_CS});
+            if (wg == 0) mma_frag<N::AP, 1, 1, 8>(dWh, MmaOperand{uA3, 256, 128, ACS}, MmaOperand{uDH, 256, 128, ACS});
+            bias_colsum<N::AP / 8>(sDH, tid, sBh);     // bias grad of the heads
+            uint32_t ua[8];
+            load_act_frag<32, false>(ua, sA3, off3);
+            wgmma_wait<0>();
+            TSTAMP();   // MMA a done
+            delta_epilogue<32>(d, ua, sD3, nullptr, off3);      // d3 = d3pre * act'(a3)
         }
         fence_async_smem();
         __syncthreads();
         TSTAMP();   // d3 epilogue done
-        // ---- d2pre = d3 . W3 ; dW3^T += a2^T . d3 ----
-        mma128<N::U2, 0, 1, 2>(TT, N::U3 / 16, false, [&](int k, uint64_t& a, uint64_t& b) {
-            a = make_smem_desc(smem_u32(sD3) + k * 2 * N::ACS, N::ACS, N::ARS);
-            b = make_smem_desc(smem_u32(sW3) + k * 256, 128, N::W3_CS);
-        });
-        mma128<N::U3, 1, 1, 2>(TW3, 8, !first, [&](int k, uint64_t& a, uint64_t& b) {
-            a = make_smem_desc(smem_u32(sA2) + k * 256, 128, N::ACS);
-            b = make_smem_desc(smem_u32(sD3) + k * 256, 128, N::ACS);
-        });
-        colsum8<128, N::U3 / 8, N::ACS, 256>(sD3, tid, bsum3);
-        TSTAMP();   // MMA b done
-        {   // d2 = d2pre * elu'(a2): U2/2 = 64 columns per thread
-            uint8_t* g2 = p.delta2 + (size_t)tile * N::A2_BYTES;
-#pragma unroll 1
-            for (int c0 = h * (N::U2 / 2); c0 < (h + 1) * (N::U2 / 2); c0 += 32) {
-                float v[32];
-                tmem_ld32(TT + lane_base + c0, v);
+        {   // ---- d2pre = d3 . W3 ; dW3^T += a2^T . d3 ----
+            float d[32];
 #pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    float a[8];
-                    unpack8_bf16(*reinterpret_cast<const uint4*>(sA2 + tile_off(row, c0 / 8 + g, N::ACS, N::ARS)), a);
-                    mul_act_grad8(&v[g * 8], a);
-                }
-                store_chunks32(v, row, c0, sD2, g2);
-            }
+            for (int j = 0; j < 32; ++j) d[j] = 0.f;
+            mma_frag<64, 0, 1, N::U3 / 16>(d, MmaOperand{uD3 + mh * 8 * ARS, 2 * ACS, ACS, ARS}, MmaOperand{uW3 + nh * 8 * N::W3_CS, 256, 128, N::W3_CS});
+            mma_frag<32, 1, 1, 8>(dW3, MmaOperand{uA2 + mh * 8 * ACS, 256, 128, ACS}, MmaOperand{uD3 + nh * 4 * ACS, 256, 128, ACS});
+            bias_colsum<N::U3 / 8>(sD3, tid, sB3);
+            uint32_t ua[16];
+            load_act_frag<64, false>(ua, sA2, off2);
+            wgmma_wait<0>();
+            TSTAMP();   // MMA b done
+            delta_epilogue<64>(d, ua, sD2, p.delta2 + (size_t)tile * N::A2_BYTES, off2);      // d2 = d2pre * act'(a2)
         }
         fence_async_smem();
         __syncthreads();
         TSTAMP();   // d2 epilogue done
-        // ---- d1pre = d2 . W2 ----
-        if (tid == 0) {
-            if (tile + (int)gridDim.x < n_tiles) {
-                // d_head / a3 / a2 tiles are dead (MMAs a, b completed, epilogue reads fenced + synced): prefetch the next tile's
-                // operands so that they land while d1pre and its 128-column epilogue run
-                const int nt = tile + gridDim.x;
-                mbar_expect_tx(&bars[1], N::DH_BYTES + N::A3_BYTES + N::A2_BYTES);
-                bulk_g2s(sDH, p.dhead + (size_t)nt * N::DH_BYTES, N::DH_BYTES, &bars[1]);
-                bulk_g2s(sA3, p.act3 + (size_t)nt * N::A3_BYTES, N::A3_BYTES, &bars[1]);
-                bulk_g2s(sA2, p.act2 + (size_t)nt * N::A2_BYTES, N::A2_BYTES, &bars[1]);
-            }
+        if (tid == 0 && tile + (int)gridDim.x < n_tiles) {
+            // d_head / a3 / a2 tiles are dead (MMAs a, b completed, epilogue reads fenced + synced): prefetch the next tile's
+            // operands so that they land while d1pre and its epilogue run
+            const int nt = tile + gridDim.x;
+            mbar_expect_tx(&bars[1], N::DH_BYTES + N::A3_BYTES + N::A2_BYTES);
+            bulk_g2s(sDH, p.dhead + (size_t)nt * N::DH_BYTES, N::DH_BYTES, &bars[1]);
+            bulk_g2s(sA3, p.act3 + (size_t)nt * N::A3_BYTES, N::A3_BYTES, &bars[1]);
+            bulk_g2s(sA2, p.act2 + (size_t)nt * N::A2_BYTES, N::A2_BYTES, &bars[1]);
         }
-        mma128<N::U1, 0, 1, 2>(TT, N::U2 / 16, false, [&](int k, uint64_t& a, uint64_t& b) {
-            a = make_smem_desc(smem_u32(sD2) + k * 2 * N::ACS, N::ACS, N::ARS);
-            b = make_smem_desc(smem_u32(sW2) + k * 256, 128, N::W2_CS);
-        });
-        colsum8<128, N::U2 / 8, N::ACS, 256>(sD2, tid, bsum2);
-        TSTAMP();   // MMA c done
-        {   // d1 = d1pre * elu'(a1) straight to the global tiled buffer (a1 read from its global tile, coalesced 16B)
-            const uint8_t* ga1 = p.act1 + (size_t)tile * N::A1_BYTES;
+        {   // ---- d1pre = d2 . W2 in two column halves: the epilogue of the first runs while the chain of the second is in flight ----
+            const uint8_t* ga1 = p.act1 + (size_t)tile * N::A1_BYTES;      // a1 is read from its global tile
             uint8_t* g1 = p.delta1 + (size_t)tile * N::A1_BYTES;
-#pragma unroll 1
-            for (int c0 = h * (N::U1 / 2); c0 < (h + 1) * (N::U1 / 2); c0 += 32) {
-                uint4 ua[4];
+            float da[32], db[32];
 #pragma unroll
-                for (int g = 0; g < 4; ++g) ua[g] = __ldg(reinterpret_cast<const uint4*>(ga1 + tile_off(row, c0 / 8 + g, N::ACS, N::ARS)));
-                float v[32];
-                tmem_ld32(TT + lane_base + c0, v);
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    float a[8];
-                    unpack8_bf16(ua[g], a);
-                    mul_act_grad8(&v[g * 8], a);
-                }
-                store_chunks32(v, row, c0, nullptr, g1);
-            }
+            for (int j = 0; j < 32; ++j) { da[j] = 0.f; db[j] = 0.f; }
+            const MmaOperand a{uD2 + mh * 8 * ARS, 2 * ACS, ACS, ARS};
+            mma_frag<64, 0, 1, N::U2 / 16>(da, a, MmaOperand{uW2 + (nh * 16) * N::W2_CS, 256, 128, N::W2_CS});
+            mma_frag<64, 0, 1, N::U2 / 16>(db, a, MmaOperand{uW2 + (nh * 16 + 8) * N::W2_CS, 256, 128, N::W2_CS});
+            bias_colsum<N::U2 / 8>(sD2, tid, sB2);
+            uint32_t ua[16];
+            load_act_frag<64, true>(ua, ga1, off1);
+            wgmma_wait<1>();
+            TSTAMP();   // first half of MMA c done
+            delta_epilogue<64>(da, ua, nullptr, g1, off1);      // d1 = d1pre * act'(a1) straight to the global tile
+            load_act_frag<64, true>(ua, ga1, off1 + 8 * ACS);
+            wgmma_wait<0>();
+            delta_epilogue<64>(db, ua, nullptr, g1, off1 + 8 * ACS);
         }
-        __syncthreads();
         TSTAMP();   // d1 epilogue done
+        // no barrier here: the next writers of sD3 / sD2 come after the next tile's barriers, and every warpgroup has waited for its MMAs
         phase ^= 1;
         first = false;
     }
     if (first) mbar_wait(&bars[0], 0);
-    // ---- flush: dW3^T (accumulator lanes = in index, cols = out index), dWh^T, bias sums ----
+    // ---- flush: dW3^T, dWh^T (rows = in index, cols = out index) with the LOGICAL strides of the parameter arena, bias sums ----
+    __syncthreads();      // the bias sums of the last tile are visible to the threads that write them out
     float* part = p.part + (size_t)blockIdx.x * p.P;
-    const bool native = p.u1 == N::U1 && p.u2 == N::U2 && p.u3 == N::U3;
-    if (!first) {
-        {   // dW3^T[i][o] -> grad_W3[o * U2 + i]; thread row = i, cols [32h, 32h+32) of U3 = 64
-            const int c0 = h * (N::U3 / 2);
-            float v[32];
-            tmem_ld32(TW3 + lane_base + c0, v);
-            if (native) {          // compile-time strides (immediate offsets): the path of the [256,128,64] geometry
-#pragma unroll
-                for (int j = 0; j < 32; ++j) part[p.off_W3 + (c0 + j) * N::U2 + row] = v[j];
-            } else if (row < p.u2) {
-                float* dst = part + p.off_W3 + c0 * p.u2 + row;
-                const int nv = p.u3 - c0;
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (j < nv) dst[j * p.u2] = v[j];
-            }
-        }
-        if (h == 0) {   // dWh^T[i][o]: rows i < u3 valid; grad_Wh[o * u3 + i], o < A + 1
-            // every lane of the h == 0 warps reads its lane, whatever u3 is; only the stores are predicated
-            float v[16];
-            tmem_ld16(TWH + lane_base, v);
-            if (row < p.u3) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    if (j < p.A + 1) part[p.off_Wh + j * p.u3 + row] = v[j];
-            }
-        }
-    } else {
-        for (int i = tid; i < p.u3 * p.u2; i += 256) part[p.off_W3 + i] = 0.f;
-        for (int i = tid; i < (p.A + 1) * p.u3; i += 256) part[p.off_Wh + i] = 0.f;
-    }
-    {
-        int g = colsum8_owner_group<N::U3 / 8, 256>(tid);
-        if (g >= 0) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                if (g * 8 + j < p.u3) part[p.off_b3 + g * 8 + j] = bsum3[j];
-        }
-        g = colsum8_owner_group<N::U2 / 8, 256>(tid);
-        if (g >= 0) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                if (g * 8 + j < p.u2) part[p.off_b2 + g * 8 + j] = bsum2[j];
-        }
-        g = colsum8_owner_group<N::AP / 8, 256>(tid);
-        if (g >= 0) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                if (g * 8 + j < p.A + 1) part[p.off_bh + g * 8 + j] = bsumh[j];
-        }
-    }
+    flush_frag<32>(dW3, part + p.off_W3, p.u2, 64 * mh + frag_row(), 32 * nh + fc, p.u2, p.u3);      // grad_W3[o * u2 + i]
+    if (wg == 0) flush_frag<N::AP>(dWh, part + p.off_Wh, p.u3, frag_row(), fc, p.u3, p.A + 1);        // grad_Wh[o * u3 + i]
+    flush_bias(sB3, p.u3, part + p.off_b3, tid);
+    flush_bias(sB2, p.u2, part + p.off_b2, tid);
+    flush_bias(sBh, p.A + 1, part + p.off_bh, tid);
     __syncthreads();
     TSTAMP();   // flush done
     TSTAMP_END();
 }
 
-// accumulator columns of the backward kernels: warp 0 takes all 512 columns, every thread learns the base
+// accumulator columns of the layer-1 weight-gradient kernel: warp 0 takes all 512 columns, every thread learns the base
 __device__ __forceinline__ uint32_t bwd_tmem_alloc(uint32_t* slot) {
     if ((threadIdx.x >> 5) == 0) tmem_alloc(slot, 512);
     __syncthreads();
@@ -1031,11 +1019,9 @@ __device__ __forceinline__ uint32_t bwd_tmem_alloc(uint32_t* slot) {
 }
 
 template <class N>
-__global__ void __launch_bounds__(256, 1) mlp_bwd1_tc_kernel(const Bwd1Args p) {
+__global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd1_tc_kernel(const Bwd1Args p) {
     extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ uint32_t tmem_slot;
-    const uint32_t tmem = bwd_tmem_alloc(&tmem_slot);
-    bwd1_body<N>(p, smem, tmem);
+    bwd1_body<N>(p, smem);
 }
 
 // ================================================================================================= backward 2
@@ -1049,40 +1035,41 @@ struct Bwd2Args {
 
 // XL1 (wide observations): dW1 is l1_wgrad_tc_kernel's job -- no X tile, no dW1^T accumulator, no W1 flush here (db1 stays).
 template <class N, bool XL1 = false>
-__device__ __forceinline__ void bwd2_body(const Bwd2Args& p, uint8_t* smem, const uint32_t tmem) {
-    // dW2^T[i][o] = sum_r a1[r][i] d2[r][o]   (two M = 128 halves over i, N = U2)      -> grad_W2[o*U1 + i]
-    // dW1^T[i][o] = sum_r x[r][i]  d1[r][o]   (x tile zero-padded to 128 columns, N = U1) -> grad_W1[o*D + i]
-    // Accumulator lanes carry the contiguous `in` index, so the flush stores are coalesced.
-    uint8_t* sD2 = smem; uint8_t* sD1 = sD2 + N::A2_BYTES; uint8_t* sA1 = sD1 + N::A1_BYTES; uint8_t* sX = sA1 + N::A1_BYTES;   // sX: 128 cols
-    float* sNorm = reinterpret_cast<float*>(sX + (XL1 ? 0 : 128 * 256));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sNorm + (XL1 ? 0 : 2 * N::DPAD));          // [0] tile loads, [1] mma
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int q = warp & 3, h = warp >> 2;
-    const int row = q * 32 + lane;
+__device__ __forceinline__ void bwd2_body(const Bwd2Args& p, uint8_t* smem) {
+    // dW2^T[i][o] = sum_r a1[r][i] d2[r][o]   (warpgroup wg: in rows [64 wg, +64), N = U2)              -> grad_W2[o*U1 + i]
+    // dW1^T[i][o] = sum_r x[r][i]  d1[r][o]   (M = DPAD = 64 in rows, warpgroup wg: out columns [64 wg, +64)) -> grad_W1[o*D + i]
+    // Both stay in registers over the whole tile loop.
+    static_assert(XL1 || N::DPAD == 64, "dW1^T is one M = 64 MMA over the padded observation columns");
+    uint8_t* sD2 = smem; uint8_t* sD1 = sD2 + N::A2_BYTES; uint8_t* sA1 = sD1 + N::A1_BYTES; uint8_t* sX = sA1 + N::A1_BYTES;
+    float* sNorm = reinterpret_cast<float*>(sX + (XL1 ? 0 : N::X_BYTES));
+    float* sB1 = sNorm + (XL1 ? 0 : 2 * N::DPAD);                                            // running bias-gradient sums
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sB1 + N::U1);                              // [0] tile loads
+    const int tid = threadIdx.x, wg = tid >> 7;
     const int n_tiles = (p.M + 127) / 128;
     int n_stamp = 0; (void)n_stamp;
     constexpr int TSB = 256; (void)TSB;
     TSTAMP();   // kernel start
     if (tid == 0) {
-        mbar_init(&bars[0], 1); mbar_init(&bars[1], 1);
+        mbar_init(&bars[0], 1);
         fence_mbar_init();
     }
     pdl_sync();
     const bool x_from_fwd = !XL1 && p.xt != nullptr;     // the forward kernel's bf16 X tile arrives by TMA with the delta tiles
     if constexpr (!XL1) {
-    if (!x_from_fwd) load_norm_smem<N>(sNorm, p.nm, p.ns, p.D);
-    for (int i = tid; i < (128 * 256 - (int)N::X_BYTES) / 16; i += 256) reinterpret_cast<uint4*>(sX + N::X_BYTES)[i] = make_uint4(0, 0, 0, 0);
+        if (!x_from_fwd) load_norm_smem<N>(sNorm, p.nm, p.ns, p.D);
     }
-    fence_async_smem();
-    __syncthreads();
-    const uint32_t TW2 = tmem, TW1 = tmem + 256;     // dW2^T halves [128 x U2] at +0, +128 ; dW1^T [128 x U1] at +256
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    float bsum1[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int i = tid; i < N::U1; i += BWD_THREADS) sB1[i] = 0.f;
+    constexpr uint32_t ACS = N::ACS;
+    const uint32_t uD2 = smem_u32(sD2), uD1 = smem_u32(sD1), uA1 = smem_u32(sA1), uX = smem_u32(sX);
+    float dW2[N::U2 / 2], dW1[XL1 ? 1 : 32];
+#pragma unroll
+    for (int j = 0; j < N::U2 / 2; ++j) dW2[j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < (XL1 ? 1 : 32); ++j) dW1[j] = 0.f;
     uint32_t phase = 0;
-    bool first = true;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        __syncthreads();
-        TSTAMP();   // tile start (previous MMAs done)
+        __syncthreads();      // the previous tile's MMAs (every warpgroup waited for its own) and bias sums have read the operand tiles
+        TSTAMP();   // tile start
         if (tid == 0) {
             mbar_expect_tx(&bars[0], N::A2_BYTES + 2 * N::A1_BYTES + (x_from_fwd ? N::X_BYTES : 0u));
             bulk_g2s(sD2, p.delta2 + (size_t)tile * N::A2_BYTES, N::A2_BYTES, &bars[0]);
@@ -1091,86 +1078,33 @@ __device__ __forceinline__ void bwd2_body(const Bwd2Args& p, uint8_t* smem, cons
             if (x_from_fwd) bulk_g2s(sX, p.xt + (size_t)tile * N::X_BYTES, N::X_BYTES, &bars[0]);
         }
         if constexpr (!XL1) {
-        if (!x_from_fwd) {
-        const int m0 = tile * 128;
-        stage_x_tile<N, 256>(sX, p.obs, chunk_row(m0, p.rows_per_chunk, p.chunk_stride), min(128, p.M - m0), p.D, sNorm, p.nm != nullptr);
-        fence_async_smem();
-        }
+            if (!x_from_fwd) {
+                const int m0 = tile * 128;
+                // one 32-byte item per thread and pass: the accumulators leave few registers for loads in flight
+#pragma unroll 1
+                for (int cg = 0; cg < N::DPAD / 8; cg += 4)
+                    stage_x_cols<N, BWD_THREADS, 4>(sX, p.obs, chunk_row(m0, p.rows_per_chunk, p.chunk_stride), min(128, p.M - m0), p.D, sNorm,
+                                                    p.nm != nullptr, cg, tid);
+                fence_async_smem();
+            }
         }
         TSTAMP();   // X staged
         mbar_wait(&bars[0], phase);
         __syncthreads();
         TSTAMP();   // tile loads landed
-        for (int hh = 0; hh < N::U1 / 128; ++hh)
-            mma128<N::U2, 1, 1, 2>(TW2 + hh * N::U2, 8, !first, [&](int k, uint64_t& a, uint64_t& b) {
-                a = make_smem_desc(smem_u32(sA1) + hh * 16 * N::ACS + k * 256, 128, N::ACS);
-                b = make_smem_desc(smem_u32(sD2) + k * 256, 128, N::ACS);
-            });
-        if constexpr (!XL1)
-            mma128<N::U1, 1, 1, 2>(TW1, 8, !first, [&](int k, uint64_t& a, uint64_t& b) {
-                a = make_smem_desc(smem_u32(sX) + k * 256, 128, N::ACS);
-                b = make_smem_desc(smem_u32(sD1) + k * 256, 128, N::ACS);
-            });
-        colsum8<128, N::U1 / 8, N::ACS, 256>(sD1, tid, bsum1);
-        TSTAMP();   // bias sums done
+        mma_frag<N::U2, 1, 1, 8>(dW2, MmaOperand{uA1 + wg * 8 * ACS, 256, 128, ACS}, MmaOperand{uD2, 256, 128, ACS});
+        if constexpr (!XL1) mma_frag<64, 1, 1, 8>(dW1, MmaOperand{uX, 256, 128, ACS}, MmaOperand{uD1 + wg * 8 * ACS, 256, 128, ACS});
+        bias_colsum<N::U1 / 8, 1>(sD1, tid, sB1);
+        wgmma_wait<0>();
+        TSTAMP();   // MMAs and bias sums done
         phase ^= 1;
-        first = false;
     }
+    __syncthreads();      // the bias sums of the last tile are visible to the threads that write them out
+    TSTAMP();   // last MMAs done
     float* part = p.part + (size_t)blockIdx.x * p.P;
-    const bool native = p.u1 == N::U1 && p.u2 == N::U2;
-    if (!first) {
-        TSTAMP();   // last MMAs done
-        // dW2^T halves: lane = in index i (hh*128 + row), columns = out o: thread takes o in [64h, 64h+64)
-#pragma unroll 1
-        for (int hh = 0; hh < N::U1 / 128; ++hh) {
-#pragma unroll 1
-            for (int c0 = h * (N::U2 / 2); c0 < (h + 1) * (N::U2 / 2); c0 += 32) {
-                float v[32];
-                tmem_ld32(TW2 + hh * N::U2 + lane_base + c0, v);
-                if (native) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) part[p.off_W2 + (size_t)(c0 + j) * N::U1 + hh * 128 + row] = v[j];
-                } else if (hh * 128 + row < p.u1) {
-                    float* dst = part + p.off_W2 + c0 * p.u1 + hh * 128 + row;
-                    const int nv = p.u2 - c0;
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (j < nv) dst[j * p.u1] = v[j];
-                }
-            }
-        }
-        // dW1^T: lane = in index i = row (< D valid), columns = out o in [128h, 128h+128)
-        if constexpr (!XL1) {
-#pragma unroll 1
-        for (int c0 = h * (N::U1 / 2); c0 < (h + 1) * (N::U1 / 2); c0 += 32) {
-            float v[32];
-            tmem_ld32(TW1 + lane_base + c0, v);
-            if (row < p.D) {
-                float* dst = part + p.off_W1 + c0 * p.D + row;
-                if (native) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) dst[j * p.D] = v[j];
-                } else {
-                    const int nv = p.u1 - c0;
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (j < nv) dst[j * p.D] = v[j];
-                }
-            }
-        }
-        }
-    } else {
-        for (int i = tid; i < p.u2 * p.u1; i += 256) part[p.off_W2 + i] = 0.f;
-        if (!XL1) for (int i = tid; i < p.u1 * p.D; i += 256) part[p.off_W1 + i] = 0.f;
-    }
-    {
-        const int g = colsum8_owner_group<N::U1 / 8, 256>(tid);
-        if (g >= 0) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                if (g * 8 + j < p.u1) part[p.off_b1 + g * 8 + j] = bsum1[j];
-        }
-    }
+    flush_frag<N::U2>(dW2, part + p.off_W2, p.u1, 64 * wg + frag_row(), frag_col(), p.u1, p.u2);
+    if constexpr (!XL1) flush_frag<64>(dW1, part + p.off_W1, p.D, frag_row(), 64 * wg + frag_col(), p.D, p.u1);
+    flush_bias(sB1, p.u1, part + p.off_b1, tid);
     __syncthreads();
     TSTAMP();   // flush done
     TSTAMP_END();
@@ -1183,16 +1117,14 @@ __device__ __forceinline__ void bwd2_body(const Bwd2Args& p, uint8_t* smem, cons
 struct BwdArgs { Bwd1Args a; Bwd2Args b; };
 
 template <class N, bool XL1 = false>
-__global__ void __launch_bounds__(256, 1) mlp_bwd_tc_kernel(const BwdArgs p) {
+__global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_tc_kernel(const BwdArgs p) {
     extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ uint32_t tmem_slot;
-    const uint32_t tmem = bwd_tmem_alloc(&tmem_slot);
-    bwd1_body<N>(p.a, smem, tmem);
+    bwd1_body<N>(p.a, smem);
     __threadfence();
     asm volatile("fence.proxy.async.global;" ::: "memory");
     fence_async_smem();          // phase 2 re-uses the shared memory of phase 1 as TMA destinations
     __syncthreads();
-    bwd2_body<N, XL1>(p.b, smem, tmem);
+    bwd2_body<N, XL1>(p.b, smem);
 }
 
 // ---- backward 2, pipelined edition: the row index is the GEMM K dimension here, so the 128-row tiles are consumed as 64-row
@@ -1495,11 +1427,12 @@ template <class N, bool XL1 = false> constexpr size_t fwd_smem() {
 template <class N> constexpr size_t l1_fwd_smem() { return (size_t)N::W1_BYTES + N::X_BYTES + sizeof(float) * (N::U1 + 2 * N::DPAD) + 2 * 8 + 16; }
 template <class N> constexpr size_t l1_wgrad_smem() { return (size_t)N::A1_BYTES + N::X_BYTES + sizeof(float) * 2 * N::DPAD + 2 * 8 + 16; }
 template <class N> constexpr size_t bwd1_smem() {
-    return (size_t)N::WH_BYTES + N::W3_BYTES + N::W2_BYTES + N::DH_BYTES + 128 * 256 + N::A2_BYTES + N::A3_BYTES + N::A2_BYTES + 8 * 8 + 16;
+    return (size_t)N::WH_BYTES + N::W3_BYTES + N::W2_BYTES + N::DH_BYTES + N::A3_BYTES + N::A2_BYTES + N::A3_BYTES + N::A2_BYTES +
+           sizeof(float) * (N::AP + N::U3 + N::U2) + 2 * 8 + 16;
 }
 template <class N> constexpr size_t bwd2_db_smem() { return (size_t)2 * (N::A2_BYTES / 2 + N::A1_BYTES + 16 * 1024) + 4 * 8 + 16; }
 template <class N, bool XL1 = false> constexpr size_t bwd2_smem() {
-    return (size_t)N::A2_BYTES + 2 * N::A1_BYTES + (XL1 ? 0 : 128 * 256 + sizeof(float) * 2 * N::DPAD) + 4 * 8 + 16;
+    return (size_t)N::A2_BYTES + 2 * N::A1_BYTES + (XL1 ? 0 : N::X_BYTES + sizeof(float) * 2 * N::DPAD) + sizeof(float) * N::U1 + 8 + 16;
 }
 template <class N, bool XL1 = false> constexpr size_t bwd_smem() {
     return bwd1_smem<N>() > bwd2_smem<N, XL1>() ? bwd1_smem<N>() : bwd2_smem<N, XL1>();
@@ -1743,7 +1676,7 @@ extern "C" int TCIMPL(b200rl_tcimpl_bwd)(const float* obs, int rows_per_chunk, i
         static_assert(smem1 <= 227 * 1024, "bwd1 shared memory budget");
         e = cudaFuncSetAttribute(mlp_bwd1_tc_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1);
         if (e != cudaSuccess) return (int)e;
-        e = launch_k(mlp_bwd1_tc_kernel<N>, dim3(grid), dim3(256), smem1, as_stream(stream), a);
+        e = launch_k(mlp_bwd1_tc_kernel<N>, dim3(grid), dim3(BWD_THREADS), smem1, as_stream(stream), a);
         if (e != cudaSuccess) return (int)e;
         Bwd2DbArgs b{(const uint8_t*)xtile, (const uint8_t*)act1, (const uint8_t*)delta2, (const uint8_t*)delta1, part, M, D, P,
                      off_W2, off_W1, off_b1};
@@ -1763,7 +1696,7 @@ extern "C" int TCIMPL(b200rl_tcimpl_bwd)(const float* obs, int rows_per_chunk, i
         static_assert(smemw <= 227 * 1024, "backward kernel (external layer 1) shared memory budget");
         e = cudaFuncSetAttribute(mlp_bwd_tc_kernel<NetW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemw);
         if (e != cudaSuccess) return (int)e;
-        e = launch_k(mlp_bwd_tc_kernel<NetW, true>, dim3(grid), dim3(256), smemw, as_stream(stream), abw);
+        e = launch_k(mlp_bwd_tc_kernel<NetW, true>, dim3(grid), dim3(BWD_THREADS), smemw, as_stream(stream), abw);
         if (e != cudaSuccess) return (int)e;
         L1WgradArgs w{obs, rows_per_chunk, chunk_stride, D, norm_mean, norm_std, (const uint8_t*)delta1, part, M, P, off_W1, u1, (const uint8_t*)xtile};
         constexpr size_t smem1w = l1_wgrad_smem<NetW>();
@@ -1780,7 +1713,7 @@ extern "C" int TCIMPL(b200rl_tcimpl_bwd)(const float* obs, int rows_per_chunk, i
     static_assert(smem <= 227 * 1024, "backward kernel shared memory budget");
     e = cudaFuncSetAttribute(mlp_bwd_tc_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
-    e = launch_k(mlp_bwd_tc_kernel<N>, dim3(grid), dim3(256), smem, as_stream(stream), ab);
+    e = launch_k(mlp_bwd_tc_kernel<N>, dim3(grid), dim3(BWD_THREADS), smem, as_stream(stream), ab);
     if (e != cudaSuccess) return (int)e;
     return B200RL_OK;
 }

@@ -1,6 +1,6 @@
-// Hopper (sm_90a) tensor-core building blocks: wgmma on shared-memory operand descriptors, mbarrier, and the per-CTA fp32
-// accumulator buffer that the fused MLP kernels address by (lane, column).  Descriptor bit layouts follow the PTX ISA's
-// wgmma matrix descriptor (the same fields CUTLASS's GmmaDescriptor names).
+// Hopper (sm_90a) tensor-core building blocks: wgmma on shared-memory operand descriptors, mbarrier, the register-accumulator chain
+// of the fused backward kernels (mma_frag) and the per-CTA fp32 accumulator buffer that the other fused MLP kernels address by
+// (lane, column).  Descriptor bit layouts follow the PTX ISA's wgmma matrix descriptor (the same fields CUTLASS's GmmaDescriptor names).
 //
 // Shared-memory operand tiles use the canonical INTERLEAVE (no-swizzle) layout: 16-byte chunks of 8 bf16
 // that are contiguous along the tile's "column" index, 8 consecutive "rows" stacked at 16 B stride (one 128 B
@@ -107,6 +107,26 @@ __device__ __forceinline__ void wgmma_m64(float (&d)[NS / 2], uint64_t a, uint64
     else if constexpr (NS == 64) wgmma_m64n64<TA, TB>(d, a, b);
     else { static_assert(NS == 128, "wgmma tile width"); wgmma_m64n128<TA, TB>(d, a, b); }
 }
+
+// ---- register-accumulator MMA -----------------------------------------------------------------------------------
+// One operand of a wgmma chain, as seen by the calling warpgroup: 32-bit shared address of its sub-tile at k = 0 (any offset along
+// M/N already folded in: 64-bit descriptor arithmetic between chained wgmmas makes ptxas serialise them), byte step per k step of
+// 16 reduction elements, and the two descriptor strides.
+struct MmaOperand { uint32_t addr, kstep, lbo, sbo; };
+// d[64 x NS] += sum over k < NK of A_k[64 x 16] . B_k[16 x NS] on a fragment the calling warpgroup owns.  Issues and commits the chain
+// and returns: no wait, no global memory, no barrier.  d must not be touched before a wgmma_wait<> that covers this group.
+template <int NS, int TA, int TB, int NK>
+__device__ __forceinline__ void mma_frag(float (&d)[NS / 2], const MmaOperand a, const MmaOperand b) {
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < NK; ++k)
+        wgmma_m64<NS, TA, TB>(d, make_smem_desc(a.addr + k * a.kstep, a.lbo, a.sbo), make_smem_desc(b.addr + k * b.kstep, b.lbo, b.sbo));
+    wgmma_commit();
+}
+// fragment -> tile coordinates: d[4j], d[4j+1] sit at row frag_row(), columns 8j + frag_col() + {0, 1}; d[4j+2], d[4j+3] 8 rows below.
+// The 32 lanes of a warp cover 8 rows x 4 column pairs per j = one 128-byte core matrix of an INTERLEAVE tile.
+__device__ __forceinline__ int frag_row() { return 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2); }
+__device__ __forceinline__ int frag_col() { return 2 * (threadIdx.x & 3); }
 
 // ---- per-CTA accumulator buffer ------------------------------------------------------------------------------
 // The fused kernels keep 128-row fp32 accumulators addressed as (lane, column) with taddr = (lane << 16) | column: layer outputs

@@ -15,9 +15,9 @@ sys.path.insert(0, ROOT)
 LABELS = {
     'fwd': ['tile start', 'X staged', 'MMA1 done', 'epi1 done', 'MMA2 done', 'epi2 done', 'MMA3 done', 'epi3 done', 'MMA4 done',
             'lossA done', 'lossB done'],
-    'bwd1': ['tile start', 'loads landed', 'MMA a done', 'd3 epi done', 'MMA b done', 'd2 epi done', 'MMA c done', 'd1 epi done'],
+    'bwd1': ['tile start', 'loads landed', 'MMA a done', 'd3 epi done', 'MMA b done', 'd2 epi done', 'MMA c half done', 'd1 epi done'],
     'bwd2': ['half start', 'loads landed', 'half done'],
-    'bwd2_old': ['tile start', 'X staged', 'loads landed', 'bias sums done'],
+    'bwd2_old': ['tile start', 'X staged', 'loads landed', 'MMAs+bias done'],
 }
 TAIL = {'fwd': ['kernel end'], 'bwd1': ['flush done'], 'bwd2': ['last MMAs done', 'flush done'], 'bwd2_old': ['last MMAs done', 'flush done']}
 
