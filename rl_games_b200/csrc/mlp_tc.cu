@@ -7,9 +7,9 @@
 //   bwd1          : delta chain d_head -> d3 -> d2 -> d1 (dgrad) + weight grads of the head and layer 3 + bias grads.
 //   bwd2          : weight grads of layers 2 and 1 (+ bias grad of layer 1).
 //
-// All GEMMs are M = 128-row wgmma chains run by every warpgroup of the CTA.  The backward kernels (bwd1 / bwd2 bodies) keep their fp32
-// accumulators in the warpgroups' registers (tc::mma_frag); the forward, the layer-1 kernels and the pipelined bwd2 use tc::mma128 (fp32
-// accumulators in the per-CTA accumulator buffer, addressed by lane = row and column like tensor memory, read back one row per thread).
+// All GEMMs are M = 128-row wgmma chains run by every warpgroup of the CTA.  The forward and backward kernels and l1_fwd keep their fp32
+// accumulators in the warpgroups' registers (tc::mma_frag); l1_wgrad and the pipelined bwd2 use tc::mma128 (fp32 accumulators in the
+// per-CTA accumulator buffer, addressed by lane = row and column like tensor memory, read back one row per thread).
 // Operands are INTERLEAVE shared-memory tiles (tc_common.cuh).  One packed bf16 copy of each weight matrix serves the forward
 // (K-major view) and the dgrad (MN-major view); one copy of each activation / delta tile serves the dgrad
 // (K-major) and the wgrad (MN-major) MMAs -- no transposes anywhere.  Tiles move global<->shared with
@@ -38,7 +38,7 @@ constexpr int TC_ACT = B200RL_TC_ACT;
 
 using namespace tc;
 
-constexpr int FWD_THREADS = 512;   // 16 warps: lane-quarter q = warp & 3 (accumulator lanes 32q..32q+31), column slice h = warp >> 2 (4 slices)
+constexpr int FWD_THREADS = 512;   // 4 warpgroups for the MMAs; the loss / rollout epilogues: row 32 (warp & 3) + lane, action slice h = warp >> 2
 
 // ---- TMA bulk helpers ---------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -301,16 +301,52 @@ __device__ __forceinline__ int colsum8_owner_group(int tid) {
     return (tid % RS == 0 && tid / RS < G) ? tid / RS : -1;
 }
 
-// epilogue helper: thread (row r) processes 32 accumulator columns [c0, c0+32): v = elu(v + bias) -> bf16 chunks into
-// a shared operand tile and (optionally) the global tiled activation buffer
-__device__ __forceinline__ void store_chunks32(const float (&v)[32], int r, int c0, uint8_t* s_tile, uint8_t* g_tile) {
+// byte offset of the bf16 pair (row r, columns c, c + 1), c even, in a 128-row activation / delta tile
+__device__ __forceinline__ uint32_t pair_off(int r, int c) { return (uint32_t)r * 16u + (uint32_t)(c & 7) * 2u + (uint32_t)(c >> 3) * 2048u; }
+
+// a = act(d + bias) on a [64 x NS] fragment whose d[0] sits at byte offset off0 (pair_off) of the tile, rounded to bf16 pairs and stored
+// at the fragment's own positions of the shared activation tile and / or the global one; bias = the bias vector at the column of d[0].
+// The 32 lanes of a warp write one 128-byte core matrix per store (tc_common.cuh).
+template <int NS>
+__device__ __forceinline__ void act_epilogue(const float (&d)[NS / 2], const float* bias, uint8_t* sT, uint8_t* gT, uint32_t off0) {
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        const uint4 u = pack8_bf16(&v[q * 8]);
-        const uint32_t off = tile_off(r, c0 / 8 + q, 2048u, 128u);
-        if (s_tile) *reinterpret_cast<uint4*>(s_tile + off) = u;
-        if (g_tile) *reinterpret_cast<uint4*>(g_tile + off) = u;
+    for (int i = 0; i < NS / 4; ++i) {
+        float v[2] = {d[2 * i], d[2 * i + 1]};
+        bias_act<2>(v, bias + 8 * (i >> 1));
+        const __nv_bfloat162 o = __floats2bfloat162_rn(v[0], v[1]);
+        const uint32_t off = off0 + (i >> 1) * 2048u + (i & 1) * 128u;
+        if (sT) *reinterpret_cast<uint32_t*>(sT + off) = *reinterpret_cast<const uint32_t*>(&o);
+        if (gT) *reinterpret_cast<uint32_t*>(gT + off) = *reinterpret_cast<const uint32_t*>(&o);
     }
+}
+
+// The same value, opaque to the compiler.  Applied inside a tile loop to the shared addresses of the MMA operands and of the bias
+// vectors: the descriptors of every chain and the epilogues' bias addresses are loop-invariant, and the compiler would otherwise
+// compute them all once before the loop and keep them (or spill them) across it.
+__device__ __forceinline__ uint32_t opaque(uint32_t x) { asm volatile("" : "+r"(x)); return x; }
+__device__ __forceinline__ const float* opaque(const float* x) { asm volatile("" : "+l"(x)); return x; }
+
+// Layer 1 of one 128-row tile, a1 = act(X . W1^T + b1), by the four warpgroups of a 512-thread CTA: warpgroup wg takes rows
+// [64 (wg & 1), +64) and columns [128 (wg >> 1), +128) as two [64 x 64] register chains, and the epilogue of the first runs while the
+// chain of the second is in flight.  The a1 tile goes to sA1 and / or gA1 (same INTERLEAVE layout).  Returns after the calling
+// warpgroup's MMAs completed; no barrier.
+template <class N>
+__device__ __forceinline__ void layer1_frag(uint32_t uX, uint32_t uW1, const float* sB1, uint8_t* sA1, uint8_t* gA1) {
+    static_assert(N::U1 == 256, "two [64 x 64] column chains per warpgroup");
+    const int wg = threadIdx.x >> 7, mh = wg & 1, nh = wg >> 1;
+    uX = opaque(uX); uW1 = opaque(uW1); sB1 = opaque(sB1);
+    float da[32], db[32];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) { da[j] = 0.f; db[j] = 0.f; }
+    const MmaOperand a{uX + mh * 8 * N::ARS, 2 * N::ACS, N::ACS, N::ARS};
+    mma_frag<64, 0, 0, N::DPAD / 16>(da, a, MmaOperand{uW1 + (nh * 16) * 128, 2 * N::W1_CS, N::W1_CS, 128});
+    mma_frag<64, 0, 0, N::DPAD / 16>(db, a, MmaOperand{uW1 + (nh * 16 + 8) * 128, 2 * N::W1_CS, N::W1_CS, 128});
+    const int c0 = 128 * nh + frag_col();
+    const uint32_t off = opaque(pair_off(64 * mh + frag_row(), c0));
+    wgmma_wait<1>();
+    act_epilogue<64>(da, sB1 + c0, sA1, gA1, off);
+    wgmma_wait<0>();
+    act_epilogue<64>(db, sB1 + c0 + 64, sA1, gA1, off + 8 * N::ACS);
 }
 
 // head[1 + h + 4k] without dynamic register-array indexing (h is a runtime warp-group id, k an unrolled constant)
@@ -383,12 +419,18 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
     float* sNorm = sSig + 64;                            // [2*DPAD] obs mean, 1/std
     float* sRed = sNorm + 2 * N::DPAD;                   // [4 warps][LOSS_SLOTS] (only the h == 0 warps run the loss)
     double* sAcc = reinterpret_cast<double*>(sRed + 4 * LOSS_SLOTS);     // [LOSS_SLOTS] per-CTA running partial
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sAcc + LOSS_SLOTS);     // [0]=W1, [1..4]=mma stages, [5]=X prefetch, [6]=W2, [7]=W3+Wh
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sAcc + LOSS_SLOTS);     // [0]=W1, [5]=X prefetch, [6]=W2, [7]=W3+Wh
+    // the head's fp32 [128 x 16] accumulator tile, read row by row by the loss / rollout epilogue: in the dead a2 (or X) region,
+    // behind the loss scratch sPart
+    float* sHead = reinterpret_cast<float*>(sXA2 + 128 * 4 * 4 * sizeof(float));
+    static_assert(128 * 4 * 4 * sizeof(float) + 128 * N::AP * sizeof(float) <= XA2_BYTES, "loss scratch and head tile fit the a2 region");
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q = warp & 3, h = warp >> 2;
     const int row = q * 32 + lane;
+    // MMA split (layer1_frag): warpgroup wg owns rows [64 (wg & 1), +64) and the column half / quarter (wg >> 1) of each layer
+    const int wg = tid >> 7, mh = wg & 1, nh = wg >> 1;
+    const int fr = 64 * mh + frag_row(), fc = frag_col();
     const int n_tiles = (p.M + 127) / 128;
     int n_stamp = 0; (void)n_stamp;
     constexpr int TSB = 0; (void)TSB;
@@ -396,7 +438,6 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
 
     // ---- prologue, part 1: nothing here depends on the predecessor kernel (PDL: may overlap its tail) ----
     const bool x_tma = !XL1 && (p.D & 3) == 0;         // 16-byte granularity of the bulk copy
-    if (warp == 0) tmem_alloc(tmem_slot, 512);
     if (tid == 0) {
         for (int i = 0; i < 8; ++i) mbar_init(&bars[i], 1);
         fence_mbar_init();
@@ -407,7 +448,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
             bulk_g2s(sXraw, p.obs + chunk_row(m0, p.rows_per_chunk, p.chunk_stride) * p.D, bytes, &bars[5]);
         }
     }
-    TSTAMP();   // TMEM allocated (warp 0), barriers initialised, first X tile requested
+    TSTAMP();   // barriers initialised, first X tile requested
     pdl_sync();
     // ---- prologue, part 2: parameters and normaliser statistics (written by the optimiser kernel) ----
     if (tid == 0) {
@@ -453,9 +494,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
         sSig[4 * p.A] = sl; sSig[4 * p.A + 1] = en;
     }
     TSTAMP();   // prologue done
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t T1 = tmem, T2 = tmem + 256, T3 = tmem + 384, T4 = tmem + 448;     // accumulator column bases
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
+    constexpr uint32_t ACS = N::ACS, ARS = N::ARS;
     uint32_t phase = 0;
     bool weights_ready = false;
     // per-thread running loss partials over this CTA's tiles (reduced once, after the tile loop): scalars in the h == 0 threads,
@@ -470,6 +509,8 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
         const int m0 = tile * 128;
         const int rows_valid = min(128, p.M - m0);
         const int64_t arow0 = chunk_row(m0, p.rows_per_chunk, p.chunk_stride);   // tile lies inside one chunk (host-checked)
+        const uint32_t uA1 = opaque(smem_u32(sA1)), uXA2 = opaque(smem_u32(sXA2)), uA3 = opaque(smem_u32(sA3));
+        const uint32_t uW2 = opaque(smem_u32(sW2)), uW3 = opaque(smem_u32(sW3)), uWh = opaque(smem_u32(sWh));
         TSTAMP();   // tile start
         if constexpr (XL1) {
             mbar_wait(&bars[5], phase);       // a1 tile landed (async-proxy write, async-proxy reader: no generic-proxy fence needed)
@@ -489,33 +530,34 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
             uint4* gx = reinterpret_cast<uint4*>(p.xt + (size_t)tile * N::X_BYTES);
             for (int i = tid; i < (int)N::X_BYTES / 16; i += FWD_THREADS) gx[i] = reinterpret_cast<const uint4*>(sXA2)[i];
         }
-        // ---------------- layer 1: T1[128, U1] = X . W1^T ----------------
-        mma128<N::U1, 0, 0, FWD_THREADS / 128>(T1, N::DPAD / 16, false, [&](int k, uint64_t& a, uint64_t& b) {
-            a = make_smem_desc(smem_u32(sXA2) + k * 2 * N::ACS, N::ACS, N::ARS);
-            b = make_smem_desc(smem_u32(sW1) + k * 2 * N::W1_CS, N::W1_CS, 128);
-        });
-        TSTAMP();   // MMA 1 done
-        {
-            uint8_t* g1 = TRAIN ? p.act1 + (size_t)tile * N::A1_BYTES : nullptr;
-#pragma unroll 1
-            for (int c0 = h * (N::U1 / 4); c0 < (h + 1) * (N::U1 / 4); c0 += 32) {
-                float v[32];
-                tmem_ld32(T1 + lane_base + c0, v);
-                bias_act<32>(v, sB1 + c0);
-                store_chunks32(v, row, c0, sA1, g1);
-            }
-        }
+        // ---------------- layer 1: a1[128, U1] = act(X . W1^T + b1) ----------------
+        layer1_frag<N>(uXA2, smem_u32(sW1), sB1, sA1, nullptr);
         fence_async_smem();
         __syncthreads();
+        if (TRAIN && tid == 0) {      // the global a1 tile is byte for byte the shared one
+            bulk_s2g(p.act1 + (size_t)tile * N::A1_BYTES, sA1, N::A1_BYTES);
+            bulk_commit();
+        }
         }   // !XL1
-        TSTAMP();   // epilogue 1 done
-        // ---------------- layer 2: T2[128, U2] = a1 . W2^T ----------------
+        TSTAMP();   // layer 1 done
+        // ---------------- layer 2: a2[128, U2] = act(a1 . W2^T + b2), warpgroup (mh, nh): [64 x 64] ----------------
         if (tile == (int)blockIdx.x) mbar_wait(&bars[6], 0);       // W2 landed (first tile only)
-        mma128<N::U2, 0, 0, FWD_THREADS / 128>(T2, N::U1 / 16, false, [&](int k, uint64_t& a, uint64_t& b) {
-            a = make_smem_desc(smem_u32(sA1) + k * 2 * N::ACS, N::ACS, N::ARS);
-            b = make_smem_desc(smem_u32(sW2) + k * 2 * N::W2_CS, N::W2_CS, 128);
-        });
-        TSTAMP();   // MMA 2 done
+        {
+            float d[32];
+#pragma unroll
+            for (int j = 0; j < 32; ++j) d[j] = 0.f;
+            mma_frag<64, 0, 0, N::U1 / 16>(d, MmaOperand{uA1 + mh * 8 * ARS, 2 * ACS, ACS, ARS},
+                                           MmaOperand{uW2 + (nh * 8) * 128, 2 * N::W2_CS, N::W2_CS, 128});
+            wgmma_wait<0>();
+            act_epilogue<64>(d, sB2 + 64 * nh + fc, sXA2, nullptr, pair_off(fr, 64 * nh + fc));
+        }
+        if (TRAIN && !XL1 && tid == 0) bulk_wait_read0();     // the a1 copy-out has read the region the X prefetch and a3 reuse
+        fence_async_smem();
+        __syncthreads();
+        if (tid == 0 && TRAIN) {
+            bulk_s2g(p.act2 + (size_t)tile * N::A2_BYTES, sXA2, N::A2_BYTES);
+            bulk_commit();
+        }
         if (XL1 && tid == 0 && tile + (int)gridDim.x < n_tiles) {
             // a1 is dead now: fetch the next tile's a1 (a3 has its own region in this layout)
             mbar_expect_tx(&bars[5], N::A1_BYTES);
@@ -528,52 +570,40 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
             mbar_expect_tx(&bars[5], bytes);
             bulk_g2s(sXraw, p.obs + chunk_row(m1, p.rows_per_chunk, p.chunk_stride) * p.D, bytes, &bars[5]);
         }
-        {
-            uint8_t* g2 = TRAIN ? p.act2 + (size_t)tile * N::A2_BYTES : nullptr;
-#pragma unroll 1
-            for (int c0 = h * (N::U2 / 4); c0 < (h + 1) * (N::U2 / 4); c0 += 32) {
-                float v[32];
-                tmem_ld32(T2 + lane_base + c0, v);
-                bias_act<32>(v, sB2 + c0);
-                store_chunks32(v, row, c0, sXA2, g2);
-            }
-        }
-        fence_async_smem();
-        __syncthreads();
-        TSTAMP();   // epilogue 2 done
-        // ---------------- layer 3: T3[128, U3] = a2 . W3^T ----------------
+        TSTAMP();   // layer 2 done
+        // ---------------- layer 3: a3[128, U3] = act(a2 . W3^T + b3), warpgroup (mh, nh): [64 x 32] ----------------
         if (tile == (int)blockIdx.x) mbar_wait(&bars[7], 0);       // W3 and the head weights landed (first tile only)
-        mma128<N::U3, 0, 0, FWD_THREADS / 128>(T3, N::U2 / 16, false, [&](int k, uint64_t& a, uint64_t& b) {
-            a = make_smem_desc(smem_u32(sXA2) + k * 2 * N::ACS, N::ACS, N::ARS);
-            b = make_smem_desc(smem_u32(sW3) + k * 2 * N::W3_CS, N::W3_CS, 128);
-        });
-        TSTAMP();   // MMA 3 done
         {
-            uint8_t* g3 = TRAIN ? p.act3 + (size_t)tile * N::A3_BYTES : nullptr;
-            // U3/4 = 16 columns per thread
-            static_assert(N::U3 / 4 == 16, "layer-3 epilogue assumes 16 columns per column slice");
-            const int c0 = h * 16;
-            float v[16];
-            tmem_ld16(T3 + lane_base + c0, v);
-            bias_act<16>(v, sB3 + c0);
+            float d[16];
 #pragma unroll
-            for (int qq = 0; qq < 2; ++qq) {
-                const uint4 u = pack8_bf16(&v[qq * 8]);
-                const uint32_t off = tile_off(row, c0 / 8 + qq, 2048u, 128u);
-                *reinterpret_cast<uint4*>(sA3 + off) = u;
-                if (g3) *reinterpret_cast<uint4*>(g3 + off) = u;
-            }
+            for (int j = 0; j < 16; ++j) d[j] = 0.f;
+            mma_frag<32, 0, 0, N::U2 / 16>(d, MmaOperand{uXA2 + mh * 8 * ARS, 2 * ACS, ACS, ARS},
+                                           MmaOperand{uW3 + (nh * 4) * 128, 2 * N::W3_CS, N::W3_CS, 128});
+            wgmma_wait<0>();
+            act_epilogue<32>(d, sB3 + 32 * nh + fc, sA3, nullptr, pair_off(fr, 32 * nh + fc));
         }
+        if (TRAIN && tid == 0) bulk_wait_read0();     // the a2 copy-out has read the region the head tile and the loss scratch reuse
         fence_async_smem();
         __syncthreads();
-        TSTAMP();   // epilogue 3 done
-        // ---------------- heads: T4[128, AP] = a3 . Wh^T ----------------
-        mma128<N::AP, 0, 0, FWD_THREADS / 128>(T4, N::U3 / 16, false, [&](int k, uint64_t& a, uint64_t& b) {
-            a = make_smem_desc(smem_u32(sA3) + k * 2 * N::ACS, N::ACS, N::ARS);
-            b = make_smem_desc(smem_u32(sWh) + k * 2 * N::WH_CS, N::WH_CS, 128);
-        });
+        if (TRAIN && tid == 0) {
+            bulk_s2g(p.act3 + (size_t)tile * N::A3_BYTES, sA3, N::A3_BYTES);
+            bulk_commit();
+        }
+        TSTAMP();   // layer 3 done
+        // ---------------- heads: [128, AP] = a3 . Wh^T, warpgroup (mh, nh): [64 x 8] -> sHead ----------------
+        {
+            float d[4] = {0.f, 0.f, 0.f, 0.f};
+            mma_frag<8, 0, 0, N::U3 / 16>(d, MmaOperand{uA3 + mh * 8 * ARS, 2 * ACS, ACS, ARS},
+                                          MmaOperand{uWh + nh * 128, 2 * N::WH_CS, N::WH_CS, 128});
+            wgmma_wait<0>();
+            const int c = 8 * nh + fc;
+            *reinterpret_cast<float2*>(sHead + fr * N::AP + c) = make_float2(d[0], d[1]);
+            *reinterpret_cast<float2*>(sHead + (fr + 8) * N::AP + c) = make_float2(d[2], d[3]);
+        }
+        __syncthreads();
+        TSTAMP();   // head done
         if (TRAIN) {
-            // ---- PPO loss, split 4 ways: the four threads (h = 0..3) that read accumulator lane `row` each take the actions
+            // ---- PPO loss, split 4 ways: the four threads (h = 0..3) that read head row `row` each take the actions
             //      j = h, h+4, h+8, h+12; per-row sums are exchanged through shared memory (the dead a2 tile region).
             const bool live = row < rows_valid;
             const int64_t ar = arow0 + row;
@@ -589,11 +619,9 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
                     if (j < p.A) { act[k] = __ldg(p.la.actions + ar * p.A + j); omu[k] = p.la.old_mu[ar * p.A + j]; osg[k] = p.la.old_sigma[ar * p.A + j]; }
                 }
             }
-            TSTAMP();   // MMA 4 done
             float head[16];
-            tmem_ld16(T4 + lane_base, head);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) head[j] += sBh[j];
+            for (int j = 0; j < 16; ++j) head[j] = sHead[row * N::AP + j] + sBh[j];
             float* sPart = reinterpret_cast<float*>(sXA2);           // [128 rows][4 h][4]: sum z^2, kl, bound loss
             float z[4];
             {
@@ -685,9 +713,8 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
             }
         } else if (h == 0) {
             float head[16];
-            tmem_ld16(T4 + lane_base, head);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) head[j] += sBh[j];
+            for (int j = 0; j < 16; ++j) head[j] = sHead[row * N::AP + j] + sBh[j];
             const int m = m0 + row;
             if (row < rows_valid) {
                 {
@@ -767,6 +794,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
                 }
             }
         }
+        if (TRAIN && tid == 0) bulk_wait_read0();     // the a3 copy-out has read its region before the next tile rewrites it
         __syncthreads();
         TSTAMP();   // loss phase B done (tile end)
         phase ^= 1;
@@ -816,9 +844,6 @@ struct Bwd1Args {
 // [64 (wg & 1), +64) and the column half (wg >> 1) of each 128-row delta layer, and one [64 x NS] block of each weight gradient,
 // which stays in its registers over all tiles of the persistent CTA and is written once, by the flush.
 constexpr int BWD_THREADS = 512;
-
-// byte offset of the bf16 pair (row r, columns c, c + 1), c even, in a 128-row activation / delta tile
-__device__ __forceinline__ uint32_t pair_off(int r, int c) { return (uint32_t)r * 16u + (uint32_t)(c & 7) * 2u + (uint32_t)(c >> 3) * 2048u; }
 
 // The activation outputs that belong to a [64 x NS] fragment whose d[0] sits at byte offset off0 (pair_off) of the tile aT: two bf16
 // pairs per 8 columns.  The 32 lanes of a warp read one 128-byte core matrix per access (tc_common.cuh): conflict-free in shared memory,
@@ -1259,9 +1284,9 @@ __global__ void __launch_bounds__(256, 1) mlp_bwd2_db_tc_kernel(const Bwd2DbArgs
 
 // ================================================================================================= wide observations: layer 1
 // a1 = elu(norm(obs) . W1^T + b1) for 64 < D <= 256 as a kernel of its own: W1 (U1 x DPAD bf16, 128 KB) stays resident, the whole
-// normalised bf16 X tile (128 x DPAD, 64 KB) is staged per tile, one K = DPAD chain of MMAs fills T1[128, U1], and the epilogue
-// writes the bf16 a1 tile straight to the global tiled buffer the chain kernels read (act1 during training, a scratch during the
-// rollout).  Same operand layouts, descriptors and epilogue as layer 1 of mlp_fwd_tc_kernel.
+// normalised bf16 X tile (128 x DPAD, 64 KB) is staged per tile, and layer1_frag (the layer 1 of mlp_fwd_tc_kernel) writes the bf16
+// a1 tile straight from its register fragments to the global tiled buffer the chain kernels read (act1 during training, a scratch
+// during the rollout).
 struct L1FwdArgs {
     const float* obs; int rows_per_chunk; int64_t chunk_stride; int D; const float* nm; const float* ns;
     const uint8_t* wpack; const float* b1; int M; uint8_t* act1; int u1, act;
@@ -1274,15 +1299,11 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) l1_fwd_tc_kernel(const L1FwdAr
     uint8_t* sW1 = smem; uint8_t* sX = sW1 + N::W1_BYTES;
     float* sB1 = reinterpret_cast<float*>(sX + N::X_BYTES);
     float* sNorm = sB1 + N::U1;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sNorm + 2 * N::DPAD);       // [0] W1, [1] mma
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int q = warp & 3, h = warp >> 2;
-    const int row = q * 32 + lane;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sNorm + 2 * N::DPAD);       // [0] W1
+    const int tid = threadIdx.x;
     const int n_tiles = (p.M + 127) / 128;
-    if (warp == 0) tmem_alloc(tmem_slot, 256);
     if (tid == 0) {
-        mbar_init(&bars[0], 1); mbar_init(&bars[1], 1);
+        mbar_init(&bars[0], 1);
         fence_mbar_init();
     }
     pdl_sync();
@@ -1293,9 +1314,6 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) l1_fwd_tc_kernel(const L1FwdAr
     for (int i = tid; i < N::U1; i += FWD_THREADS) sB1[i] = i < p.u1 ? __ldg(p.b1 + i) : 0.f;
     load_norm_smem<N>(sNorm, p.nm, p.ns, p.D);
     __syncthreads();
-    const uint32_t T1 = *tmem_slot;
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    uint32_t phase = 0;
     bool weights_ready = false;
     constexpr int NCGP = 16;       // column groups per staging pass: 128 columns, 4 x 32 B in flight per thread
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -1312,23 +1330,9 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) l1_fwd_tc_kernel(const L1FwdAr
             bulk_s2g(p.xt + (size_t)tile * N::X_BYTES, sX, N::X_BYTES);
             bulk_commit();
         }
-        mma128<N::U1, 0, 0, FWD_THREADS / 128>(T1, N::DPAD / 16, false, [&](int k, uint64_t& a, uint64_t& b) {
-            a = make_smem_desc(smem_u32(sX) + k * 2 * N::ACS, N::ACS, N::ARS);
-            b = make_smem_desc(smem_u32(sW1) + k * 2 * N::W1_CS, N::W1_CS, 128);
-        });
-        {
-            uint8_t* g1 = p.act1 + (size_t)tile * N::A1_BYTES;
-#pragma unroll 1
-            for (int c0 = h * (N::U1 / 4); c0 < (h + 1) * (N::U1 / 4); c0 += 32) {
-                float v[32];
-                tmem_ld32(T1 + lane_base + c0, v);
-                bias_act<32>(v, sB1 + c0);
-                store_chunks32(v, row, c0, nullptr, g1);
-            }
-        }
+        layer1_frag<N>(smem_u32(sX), smem_u32(sW1), sB1, nullptr, p.act1 + (size_t)tile * N::A1_BYTES);
         if (p.xt && tid == 0) bulk_wait_read0();      // the tile's copy-out (issued before the MMAs) has finished reading sX
-        __syncthreads();       // T1 and the X tile are free for the next tile
-        phase ^= 1;
+        __syncthreads();       // every warpgroup's MMAs have read the X tile: it is free for the next tile
     }
     if (!weights_ready) mbar_wait(&bars[0], 0);
     if (p.xt && tid == 0) bulk_wait_read0();          // shared memory must outlive the last copy-out's reads

@@ -1,6 +1,6 @@
 // Hopper (sm_90a) tensor-core building blocks: wgmma on shared-memory operand descriptors, mbarrier, the register-accumulator chain
-// of the fused backward kernels (mma_frag) and the per-CTA fp32 accumulator buffer that the other fused MLP kernels address by
-// (lane, column).  Descriptor bit layouts follow the PTX ISA's wgmma matrix descriptor (the same fields CUTLASS's GmmaDescriptor names).
+// of the fused forward and backward kernels (mma_frag) and the per-CTA fp32 accumulator buffer that the remaining fused MLP kernels
+// address by (lane, column).  Descriptor bit layouts follow the PTX ISA's wgmma matrix descriptor (the same fields CUTLASS's GmmaDescriptor names).
 //
 // Shared-memory operand tiles use the canonical INTERLEAVE (no-swizzle) layout: 16-byte chunks of 8 bf16
 // that are contiguous along the tile's "column" index, 8 consecutive "rows" stacked at 16 B stride (one 128 B

@@ -13,8 +13,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 LABELS = {
-    'fwd': ['tile start', 'X staged', 'MMA1 done', 'epi1 done', 'MMA2 done', 'epi2 done', 'MMA3 done', 'epi3 done', 'MMA4 done',
-            'lossA done', 'lossB done'],
+    'fwd': ['tile start', 'X staged', 'layer 1 done', 'layer 2 done', 'layer 3 done', 'head done', 'lossA done', 'lossB done'],
     'bwd1': ['tile start', 'loads landed', 'MMA a done', 'd3 epi done', 'MMA b done', 'd2 epi done', 'MMA c half done', 'd1 epi done'],
     'bwd2': ['half start', 'loads landed', 'half done'],
     'bwd2_old': ['tile start', 'X staged', 'loads landed', 'MMAs+bias done'],
@@ -96,7 +95,7 @@ def main():
         n = buf[base]
         st = [buf[base + 1 + i] for i in range(n)]
         lab = LABELS[kind]
-        head = ['kernel start'] + (['setup (tmem, bars)', 'loads issued', 'barrier 1', 'prologue done'] if kind == 'fwd' else [])
+        head = ['kernel start'] + (['setup (bars)', 'loads issued', 'barrier 1', 'prologue done'] if kind == 'fwd' else [])
         names = head + lab * ((n - len(head) - len(TAIL[kind])) // len(lab)) + TAIL[kind]
         print('  [%s] CTA0: %d stamps, total %.1f us @1.965GHz' % (kind, n, (st[-1] - st[0]) / 1965.0))
         for i in range(1, n):
