@@ -231,6 +231,37 @@ int b200rl_ppo_head_loss_f32(const float* a_last, int Hl, const float* W_head, c
                              float* d_head, float* d_alast, int act_last,
                              float* mu_out, float* value_out, float* neglogp_out,
                              double* partials, int max_partials, int* n_blocks_out_host, void* stream);
+/* State-dependent sigma head (fixed_sigma: False, network_builder.py:324-348, :441-444) and the sigma parametrisations of
+ * models.py apply_sigma_parametrization, for a raw head output r:
+ *   B200RL_SIGMA_EXP:      r clamped to [logstd_lo, logstd_hi] if has_logstd_bounds, sigma = exp(r), logstd = r;
+ *                          min_sigma > 0: sigma = exp(r) + min_sigma, logstd = log(sigma)
+ *   B200RL_SIGMA_SOFTPLUS: sigma = softplus(r) + min_sigma (torch softplus: beta 1, threshold 20), logstd = log(sigma)
+ *   B200RL_SIGMA_LINEAR:   ('linear' / 'scalar') floor = max(min_sigma, 1e-3), sigma = floor + softplus(r - floor), logstd = log(sigma) */
+#define B200RL_SIGMA_EXP 0
+#define B200RL_SIGMA_SOFTPLUS 1
+#define B200RL_SIGMA_LINEAR 2
+typedef struct b200rl_sigma_cfg {
+    int parametrization;     /* B200RL_SIGMA_* */
+    float min_sigma;         /* space min_sigma (0 = none) */
+    int has_logstd_bounds;   /* space logstd_bounds given ('exp' only) */
+    float logstd_lo, logstd_hi;
+} b200rl_sigma_cfg;
+
+/* b200rl_ppo_head_loss_f32 for a state-dependent sigma head, A <= 15: W_head [1+2A, Hl] / b_head [1+2A] with rows
+ * (value, mu_0..A-1, raw sigma_0..A-1); sigma is per row.  d_head [M, 1+2A] = (dL/dvalue, dL/dmu, dL/draw), where dL/draw
+ * includes the entropy bonus -entropy_coef * d(entropy)/d(logstd) (entropy_coef read from device).  The partials have the same
+ * layout; their log-std slots are 0, so b200rl_ppo_loss_finalize / b200rl_reduce_finalize handed a device zero for the entropy
+ * coefficient write exactly 0 to d_logstd. */
+int b200rl_ppo_head_loss_sd_f32(const float* a_last, int Hl, const float* W_head, const float* b_head,
+                                const b200rl_sigma_cfg* sigma_cfg_host, const float* entropy_coef_dev,
+                                const float* actions, float* old_mu, float* old_sigma,
+                                const float* old_values_n, const float* returns_n, const float* old_neglogp,
+                                const float* advs_n, const float* mask,
+                                int rows_per_chunk, int64_t chunk_stride, int M, int A,
+                                const b200rl_loss_cfg* cfg_host, const float* inv_count_dev,
+                                float* d_head, float* d_alast, int act_last,
+                                float* mu_out, float* value_out, float* neglogp_out,
+                                double* partials, int max_partials, int* n_blocks_out_host, void* stream);
 /* partials -> stats[] (means; masked means when inv_count was used) and d_logstd[A]
  * (includes the -entropy_coef * d(entropy)/d(logstd) term; entropy_coef read from device). */
 int b200rl_ppo_loss_finalize(const double* partials, int n_partials, int A, const float* entropy_coef_dev,
@@ -398,6 +429,16 @@ int b200rl_policy_head_sample_f32(const float* a_last, int Hl, const float* W_he
                                   float* env_actions, int clip_actions, const float* act_low, const float* act_high,
                                   const uint8_t* dones_cur, uint8_t* dones_out, const float* prev_dones,
                                   float* valid_out, int N, int A, int values_only, void* stream);
+/* b200rl_policy_head_sample_f32 for a state-dependent sigma head (A <= 15, W_head [1+2A, Hl], see b200rl_ppo_head_loss_sd_f32):
+ * sigma per row from the raw sigma rows through sigma_cfg_host; sigmas [N,A] receives each row's sigma. */
+int b200rl_policy_head_sample_sd_f32(const float* a_last, int Hl, const float* W_head, const float* b_head,
+                                     const b200rl_sigma_cfg* sigma_cfg_host, const double* vms_mean, const double* vms_var,
+                                     int normalize_value, const float* noise, uint64_t seed,
+                                     const uint64_t* rng_epoch_dev, uint32_t step_index,
+                                     float* actions, float* mus, float* sigmas, float* neglogp, float* values,
+                                     float* env_actions, int clip_actions, const float* act_low, const float* act_high,
+                                     const uint8_t* dones_cur, uint8_t* dones_out, const float* prev_dones,
+                                     float* valid_out, int N, int A, int values_only, void* stream);
 
 typedef struct b200rl_shaper_cfg {
     float scale_value, shift_value, min_val, max_val;  /* tr_helpers.py:16-42 */

@@ -114,17 +114,21 @@ class A2CAgent(A2CBase):
         # zero-padded), elu / relu / tanh, obs <= 256, <= 15 actions; anything else runs on the fp32 kernels
         tc_ok = self.model.activation in ('elu', 'relu', 'tanh') and \
             ops.tc_supported(self.model.D, self.model.units, self.actions_num, allow_wide)
-        # (a sigma floor -- min_sigma > 0 -- is applied outside the kernels on the log-std vector they read; the fused kernels take the raw
-        #  parameter from the packed arena, so such policies run layer by layer.  Separate actor / critic trunks need their gradient mask
-        #  applied between the split reduction and the optimiser, which the fused tail does in one launch: layer by layer as well)
-        fused_ok = tc_ok and not self.is_rnn and getattr(self.model, 'min_sigma', 0.0) == 0 and not getattr(self.model, 'separate', False)
+        # (a fixed sigma other than the plain log-std -- a floor, bounds, 'softplus' / 'linear' -- is applied outside the kernels on the
+        #  log-std vector they read; the fused kernels take the raw parameter from the packed arena, so such policies run layer by layer.
+        #  Separate actor / critic trunks need their gradient mask applied between the split reduction and the optimiser, which the fused
+        #  tail does in one launch: layer by layer as well.  A state-dependent sigma head runs on the fp32 or the layer-wise tensor-core
+        #  kernels: the fused kernels have 16 head rows)
+        fused_ok = tc_ok and not self.is_rnn and not getattr(self.model, 'sigma_transform', False) and \
+            getattr(self.model, 'fixed_sigma', True) and not getattr(self.model, 'separate', False)
         if self.mixed_precision is None:
             self.mixed_precision = fused_ok
             if not self.mixed_precision and self.global_rank == 0:
                 print(f'b200: mixed_precision not set -> fp32 kernels for this geometry (obs={self.model.D}, units={self.model.units}, '
                       f'actions={self.actions_num}, activation={self.model.activation}{", rnn" if self.is_rnn else ""}); mixed_precision: True runs it '
                       f'on the tensor cores layer by layer; the FUSED bf16 wgmma kernels cover obs<=256, three-layer MLPs up to [256,128,64] '
-                      f'with elu / relu / tanh, actions<=15')
+                      f'with elu / relu / tanh, actions<=15, a fixed plain exp log-std and one shared trunk'
+                      f'{"; this state-dependent sigma head runs layer by layer either way" if not getattr(self.model, "fixed_sigma", True) else ""}')
         if self.is_rnn:
             if self.horizon_length % self.seq_length != 0:
                 raise ValueError(f"Horizon length ({self.horizon_length}) must be divisible by sequence length ({self.seq_length})")
@@ -243,7 +247,7 @@ class A2CAgent(A2CBase):
             self.ra = [f(N, u) for u in m.units]
             self.ta = [f(mb, u) for u in m.units]
             self.dA = [f(mb, u) for u in m.units]
-            self.d_head = f(mb, A + 1)
+            self.d_head = f(mb, m.head_rows)
         ops.set_pdl(self.config.get('b200_pdl', False))     # programmatic dependent launch: off by default
         if self.use_tc:
             self.n_splits = ops.NUM_SMS      # split-partial rows: at least the fused backward kernels' grid (<= one CTA per SM)
@@ -311,6 +315,9 @@ class A2CAgent(A2CBase):
         # lr, step, beta1^step, beta2^step, [KL sum, count of the running mini-epoch (schedule_type 'standard')], pad
         self.opt_state = torch.tensor([self.last_lr, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0], dtype=torch.float64, device=dev)
         self.entropy_coef_dev = torch.tensor([float(self.entropy_coef)], dtype=torch.float32, device=dev)
+        # a state-dependent sigma head takes its entropy gradient per row inside the loss kernel; the finalisation is handed this zero
+        # in place of the coefficient so that it writes exactly 0 into the dead fixed-sigma block
+        self.zero_dev = torch.zeros(1, dtype=torch.float32, device=dev)
         # linear schedule (a2c_common.py:1557-1563): the reference steps the scheduler AFTER every minibatch with the current epoch
         # number, so the first minibatch of an epoch still runs on the previous epoch's (lr, entropy_coef) and the others on this
         # epoch's.  The host knows both before the epoch starts; the switch is two device-to-device copies after the first update.
@@ -569,6 +576,14 @@ class A2CAgent(A2CBase):
         a_last = self.ra[-1]
         if self.is_rnn and not m.rnn_before_mlp:
             a_last = self._lstm_step(a_last, self.rnn_h, self.rnn_c, self.rnn_h, self.rnn_c)
+        if not m.fixed_sigma:
+            ops.policy_head_sample_sd(a_last, m.W_head, m.b_head, m.sigma_cfg, m.value_mean_std.running_mean,
+                                      m.value_mean_std.running_var, self.normalize_value, noise, self.rng_seed, self.rng_epoch, t,
+                                      self.actions[t], self.mus[t], self.sigmas[t], self.neglogpacs[t], self.values[t],
+                                      self.env_actions, self.clip_actions, self.actions_low, self.actions_high,
+                                      self.dones, self.dones_buf[t], self.prev_dones, None if self.valid is None else self.valid[t],
+                                      N, A)
+            return
         ops.policy_head_sample(a_last, m.W_head, m.b_head, m.logstd_in, m.value_mean_std.running_mean,
                                m.value_mean_std.running_var, self.normalize_value, noise, self.rng_seed, self.rng_epoch, t,
                                self.actions[t], self.mus[t], self.sigmas[t], self.neglogpacs[t], self.values[t],
@@ -593,6 +608,11 @@ class A2CAgent(A2CBase):
         a_last = self.ra[-1]
         if self.is_rnn and not m.rnn_before_mlp:
             a_last = self._lstm_step(a_last, self.rnn_h, self.rnn_c, self.r_tmp_h, self.r_tmp_c)
+        if not m.fixed_sigma:
+            ops.policy_head_sample_sd(a_last, m.W_head, m.b_head, m.sigma_cfg, m.value_mean_std.running_mean,
+                                      m.value_mean_std.running_var, self.normalize_value, None, 0, None, 0, None, None, None, None,
+                                      self.last_values, None, False, None, None, None, None, None, None, N, A, values_only=True)
+            return self.last_values.unsqueeze(1)
         ops.policy_head_sample(a_last, m.W_head, m.b_head, m.sigma, m.value_mean_std.running_mean,
                                m.value_mean_std.running_var, self.normalize_value, None, 0, None, 0, None, None, None, None,
                                self.last_values, None, False, None, None, None, None, None, None, N, A, values_only=True)
@@ -614,7 +634,7 @@ class A2CAgent(A2CBase):
         wants_infos = getattr(self.algo_observer, 'wants_infos', False)
         if hasattr(self.vec_env, 'begin_rollout'):
             self.vec_env.begin_rollout()
-        self.model.refresh_sigma_floor()          # weights may have been loaded since the last update (no-op unless min_sigma > 0)
+        self.model.refresh_sigma_floor()          # weights may have been loaded since the last update (no-op for the plain log-std)
         for t in range(H):
             obs = self.obs['obs']
             self.obses[t].copy_(obs)
@@ -744,14 +764,22 @@ class A2CAgent(A2CBase):
             a_last, d_alast, act_last = self.t_hmlp, self.t_dHmlp, 0
         else:
             a_last, d_alast, act_last = self.ta[-1], self.dA[-1], m.act_id
-        nb = ops.ppo_head_loss(a_last, m.W_head, m.b_head, m.logstd_in, self.actions[0, e0:], self.mus[0, e0:],
-                               self.sigmas[0, e0:], self.old_values_n[0, e0:], self.returns_n[0, e0:], self.neglogpacs[0, e0:],
-                               self.advs_n[0, e0:], None if self.valid is None else self.valid[0, e0:], epm, N, mb, A,
-                               self.loss_cfg, None if self.inv_counts is None else self.inv_counts[i:i + 1], self.d_head,
-                               d_alast, act_last, self.loss_partials)
         gv = self._gv[u & 1]
-        ops.ppo_loss_finalize(self.loss_partials, nb, A, self.entropy_coef_dev, self.stats[u], gv['g_sigma'], gv['kl'])
-        if m.min_sigma > 0:      # the kernels differentiated with respect to log(exp(raw) + min_sigma): chain to the raw parameter
+        if m.fixed_sigma:
+            nb = ops.ppo_head_loss(a_last, m.W_head, m.b_head, m.logstd_in, self.actions[0, e0:], self.mus[0, e0:],
+                                   self.sigmas[0, e0:], self.old_values_n[0, e0:], self.returns_n[0, e0:], self.neglogpacs[0, e0:],
+                                   self.advs_n[0, e0:], None if self.valid is None else self.valid[0, e0:], epm, N, mb, A,
+                                   self.loss_cfg, None if self.inv_counts is None else self.inv_counts[i:i + 1], self.d_head,
+                                   d_alast, act_last, self.loss_partials)
+            ops.ppo_loss_finalize(self.loss_partials, nb, A, self.entropy_coef_dev, self.stats[u], gv['g_sigma'], gv['kl'])
+        else:               # per-row sigma: the raw-sigma gradient (entropy bonus included) leaves through d_head / d_alast
+            nb = ops.ppo_head_loss_sd(a_last, m.W_head, m.b_head, m.sigma_cfg, self.entropy_coef_dev, self.actions[0, e0:],
+                                      self.mus[0, e0:], self.sigmas[0, e0:], self.old_values_n[0, e0:], self.returns_n[0, e0:],
+                                      self.neglogpacs[0, e0:], self.advs_n[0, e0:], None if self.valid is None else self.valid[0, e0:],
+                                      epm, N, mb, A, self.loss_cfg, None if self.inv_counts is None else self.inv_counts[i:i + 1],
+                                      self.d_head, d_alast, act_last, self.loss_partials)
+            ops.ppo_loss_finalize(self.loss_partials, nb, A, self.zero_dev, self.stats[u], gv['g_sigma'], gv['kl'])
+        if m.sigma_transform:    # the kernels differentiated with respect to log(sigma(raw)): chain to the raw parameter
             gv['g_sigma'].mul_(m.sigma_chain)
         P = m.num_params
         # row splits of the head / MLP weight gradients.  A recurrent policy's partial arena has seq_length x n_splits rows (one group per
@@ -759,7 +787,7 @@ class A2CAgent(A2CBase):
         S = min(self.part_rows, max(self.n_splits, mb // 256)) if self.gemm_tc else self.n_splits
         off_wh, _ = m.layout['W_head']
         off_bh, _ = m.layout['b_head']
-        self._lin_bww(self.d_head, a_last, self.part[0, off_wh:], self.part[0, off_bh:], m.Hl, A + 1, S, M=mb,
+        self._lin_bww(self.d_head, a_last, self.part[0, off_wh:], self.part[0, off_bh:], m.Hl, m.head_rows, S, M=mb,
                               split_stride=P)
         if rnn_last:
             self._lstm_window_bwd(e0)       # also fills dA[-1] = dL/d(pre-activation of the last MLP layer)
@@ -785,7 +813,7 @@ class A2CAgent(A2CBase):
         if m.grad_mask is not None:      # separate trunks: the structural zeros of the block layout get no gradient (model.py)
             gv['grad'][:P].mul_(m.grad_mask)
         self._step_optimizer(u, gv, P)
-        m.refresh_sigma_floor()          # no-op unless min_sigma > 0
+        m.refresh_sigma_floor()          # no-op for the plain log-std
 
     def _lstm_window_fwd(self, e0):
         """Training forward of the LSTM over the seq_length window of every sequence of the minibatch (network_builder.py:452-492,

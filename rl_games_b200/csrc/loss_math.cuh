@@ -18,6 +18,67 @@ __device__ __forceinline__ void loss_fill_sigma(float* sSig, const float* __rest
     sSig[j] = sg; sSig[A + j] = ls; sSig[2 * A + j] = 1.0f / sg; sSig[3 * A + j] = logf(sg);
 }
 
+// sigma parametrisations (models.py apply_sigma_parametrization); the codes of b200rl_sigma_cfg.parametrization
+constexpr int SIGMA_EXP = 0, SIGMA_SOFTPLUS = 1, SIGMA_LINEAR = 2;
+
+struct SigmaCfgDev {
+    int param, has_bounds;
+    float min_sigma, lo, hi;    // lo / hi: logstd_bounds of 'exp'
+};
+
+inline SigmaCfgDev sigma_cfg_dev(const b200rl_sigma_cfg& h) {
+    SigmaCfgDev c;
+    c.param = h.parametrization; c.has_bounds = h.has_logstd_bounds;
+    c.min_sigma = h.min_sigma; c.lo = h.logstd_lo; c.hi = h.logstd_hi;
+    return c;
+}
+
+// torch.nn.functional.softplus (beta 1, threshold 20) and its derivative
+__host__ __device__ __forceinline__ float softplus_t20(float x, float& dx) {
+    if (x > 20.0f) { dx = 1.0f; return x; }
+    const float z = expf(x);
+    dx = z / (z + 1.0f);
+    return log1pf(z);
+}
+
+// raw sigma-head output r -> sigma, logstd, and d logstd / d r (the factor that turns dL/dlogstd into dL/dr):
+//   exp:      r clamped to the bounds (gradient 1 on the closed interval, 0 outside), sigma = e^r, logstd = r;
+//             with a floor sigma = e^r + min_sigma, logstd = log(sigma)
+//   softplus: sigma = softplus(r) + min_sigma, logstd = log(sigma)
+//   linear:   floor = max(min_sigma, 1e-3), sigma = floor + softplus(r - floor), logstd = log(sigma)
+__host__ __device__ __forceinline__ void sigma_param(float r, const SigmaCfgDev& c, float& sg, float& ls, float& dls_dr) {
+    if (c.param == SIGMA_SOFTPLUS || c.param == SIGMA_LINEAR) {
+        const float floor_ = c.param == SIGMA_LINEAR ? fmaxf(c.min_sigma, 1e-3f) : c.min_sigma;
+        float dsp;
+        const float sp = softplus_t20(c.param == SIGMA_LINEAR ? r - floor_ : r, dsp);
+        sg = sp + floor_;
+        ls = logf(sg);
+        dls_dr = dsp / sg;
+        return;
+    }
+    float g = 1.0f;
+    if (c.has_bounds) {
+        g = (r >= c.lo && r <= c.hi) ? 1.0f : 0.0f;
+        r = fminf(fmaxf(r, c.lo), c.hi);
+    }
+    const float e = expf(r);
+    if (c.min_sigma > 0.0f) {
+        sg = e + c.min_sigma;
+        ls = logf(sg);
+        dls_dr = e * g / sg;
+    } else {
+        sg = e;
+        ls = r;
+        dls_dr = g;
+    }
+}
+
+// per-row sigma of a state-dependent head (one entry per action): sigma, logstd and d logstd / d raw from sigma_param
+template <int MAXA>
+struct RowSigma {
+    float sg[MAXA], ls[MAXA], dr[MAXA];
+};
+
 constexpr int LOSS_NSC = 8;   // scalar partial slots: w*a_loss, w*c_loss, w*entropy, w*b_loss, w*kl, mask, mask*clipped, w
 
 struct LossArena {
@@ -66,10 +127,14 @@ __device__ __forceinline__ void loss_row_load(const LossArena& a, int64_t ar, in
 // ar = arena row.  Outputs: dh[0] = dL/dvalue, dh[1+j] = dL/dmu_j, dls[j] = per-sample dL/dlogstd_j (without the
 // entropy term), sc[] = weighted scalar contributions; writes the new mu / sigma over the old ones
 // (datasets.py:33-43) and returns the sample's neglogp.
-template <int MAXA, bool FAST>
+// SD (state-dependent sigma, fp32 only): sigma / logstd come per row from `rs` instead of sSig, and dls[j] is the row's dL/draw_j of
+// the sigma head, the entropy bonus -ent_coef * w included (the fixed-sigma form leaves that term to the finalisation).
+template <int MAXA, bool FAST, bool SD = false>
 __device__ __forceinline__ float ppo_sample_loss(const float (&head)[MAXA], int A, const float* __restrict__ sSig,
                                                  const LossArena& ar_, int64_t ar, const LossRow<MAXA>& row, float inv_cnt,
-                                                 const LossCfgDev& cfg, float (&dh)[MAXA], float (&dls)[MAXA], float (&sc)[LOSS_NSC]) {
+                                                 const LossCfgDev& cfg, float (&dh)[MAXA], float (&dls)[MAXA], float (&sc)[LOSS_NSC],
+                                                 const RowSigma<MAXA>* rs = nullptr, float ent_coef = 0.f) {
+    static_assert(!(SD && FAST), "state-dependent sigma has no FAST form");
     const float val = head[0];
     const float old_v = row.old_v, ret = row.ret, old_nlp = row.old_nlp, adv = row.adv, mk = row.mk;
     const float w = mk * inv_cnt;
@@ -78,13 +143,13 @@ __device__ __forceinline__ float ppo_sample_loss(const float (&head)[MAXA], int 
 #pragma unroll
     for (int j = 0; j < MAXA - 1; ++j) {
         if (j < A) {
-            const float mu = head[1 + j], sg = sSig[j], ls = sSig[A + j];
+            const float mu = head[1 + j], sg = SD ? rs->sg[j] : sSig[j], ls = SD ? rs->ls[j] : sSig[A + j];
             const float act = row.act[j];
             const float omu = row.omu[j], osg = row.osg[j];
             z[j] = FAST ? (act - mu) * sSig[2 * A + j] : (act - mu) / sg;
             sumz2 += z[j] * z[j];
             sumls += ls;
-            ent += 0.5f + 0.9189385332046727f + sSig[3 * A + j];     // 0.5 + 0.5*log(2*pi) + log(sigma)
+            ent += 0.5f + 0.9189385332046727f + (SD ? logf(sg) : sSig[3 * A + j]);     // 0.5 + 0.5*log(2*pi) + log(sigma)
             const float c1 = FAST ? __logf(osg * sSig[2 * A + j] + 1e-5f) : logf(osg / sg + 1e-5f);
             const float dm = omu - mu;
             const float c2 = FAST ? (sg * sg + dm * dm) * __frcp_rn(2.0f * (osg * osg + 1e-5f))
@@ -150,7 +215,7 @@ __device__ __forceinline__ float ppo_sample_loss(const float (&head)[MAXA], int 
 #pragma unroll
     for (int j = 0; j < MAXA - 1; ++j) {
         if (j < A) {
-            const float mu = head[1 + j], sg = sSig[j];
+            const float mu = head[1 + j], sg = SD ? rs->sg[j] : sSig[j];
             float db = 0.f;
             if (cfg.has_bounds) {
                 if (cfg.bound_type == 1) db = 2.0f * fmaxf(mu - 1.1f, 0.f) + 2.0f * fminf(mu + 1.1f, 0.f);
@@ -158,6 +223,7 @@ __device__ __forceinline__ float ppo_sample_loss(const float (&head)[MAXA], int 
             }
             dh[1 + j] = w * (g_a * (FAST ? -(z[j] * sSig[2 * A + j]) : -(z[j] / sg)) + cfg.bounds_coef * db);
             dls[j] = w * g_a * (1.0f - z[j] * z[j]);
+            if (SD) dls[j] = (dls[j] - ent_coef * w) * rs->dr[j];
             ar_.old_mu[ar * A + j] = mu;          // new mu/sigma overwrite the old ones (datasets.py:33-43)
             ar_.old_sigma[ar * A + j] = sg;
         } else {

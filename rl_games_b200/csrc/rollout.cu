@@ -7,13 +7,17 @@
 //                         (a2c_common.py:1027-1051, torch_ext.py:326-352)
 //   synth_env_step     -- synthetic on-GPU measurement env (not part of the reference; SURVEY.md 8d)
 #include "common.cuh"
+#include "loss_math.cuh"
 
 namespace {
 
 constexpr int PT = 128;
 constexpr int MAXA = 32;
+constexpr int MAXA_SD = 16;   // state-dependent sigma: value + up to 15 mu rows, up to 15 raw-sigma rows
 
-__global__ void __launch_bounds__(PT) policy_head_sample_kernel(
+// SD = state-dependent sigma: 1 + 2A head rows (value, mu, raw sigma), sigma per row through sigma_param
+template <int MA, bool SD>
+__device__ __forceinline__ void policy_head_sample_body(
     const float* __restrict__ a_last, int Hl, const float* __restrict__ Wh, const float* __restrict__ bh,
     const float* __restrict__ logstd, const double* __restrict__ vms_mean, const double* __restrict__ vms_var,
     int normalize_value, const float* __restrict__ noise, uint64_t seed, const uint64_t* __restrict__ rng_epoch_dev,
@@ -21,34 +25,40 @@ __global__ void __launch_bounds__(PT) policy_head_sample_kernel(
     float* __restrict__ neglogp, float* __restrict__ values, float* __restrict__ env_actions, int clip_actions,
     const float* __restrict__ act_low, const float* __restrict__ act_high,
     const uint8_t* __restrict__ dones_cur, uint8_t* __restrict__ dones_out, const float* __restrict__ prev_dones,
-    float* __restrict__ valid_out, int N, int A, int values_only) {
+    float* __restrict__ valid_out, int N, int A, int values_only, const SigmaCfgDev& scfg) {
     extern __shared__ float smf[];
     const int AH = A + 1;
+    const int HR = SD ? 1 + 2 * A : AH;   // head rows
     float* tile = smf;                    // [PT][Hl+1]
-    float* sW = tile + PT * (Hl + 1);     // [AH][Hl]
-    float* sB = sW + AH * Hl;             // [AH]
-    float* sSig = sB + AH;                // sigma[A], logstd[A]
+    float* sW = tile + PT * (Hl + 1);     // [HR][Hl]
+    float* sB = sW + HR * Hl;             // [HR]
+    float* sSig = sB + HR;                // sigma[A], logstd[A] (fixed sigma)
     const int tid = threadIdx.x, e0 = blockIdx.x * PT;
     const int rows = min(PT, N - e0);
     for (int i = tid; i < rows * Hl; i += PT) {
         const int r = i / Hl, k = i - r * Hl;
         tile[r * (Hl + 1) + k] = __ldg(a_last + (int64_t)(e0 + r) * Hl + k);
     }
-    for (int i = tid; i < AH * Hl; i += PT) sW[i] = __ldg(Wh + i);
-    if (tid < AH) sB[tid] = __ldg(bh + tid);
-    if (tid < A) { const float ls = __ldg(logstd + tid); sSig[tid] = expf(ls); sSig[A + tid] = ls; }
+    for (int i = tid; i < HR * Hl; i += PT) sW[i] = __ldg(Wh + i);
+    if (tid < HR) sB[tid] = __ldg(bh + tid);
+    if (!SD && tid < A) { const float ls = __ldg(logstd + tid); sSig[tid] = expf(ls); sSig[A + tid] = ls; }
     __syncthreads();
     if (tid >= rows) return;
     const int e = e0 + tid;
-    float head[MAXA];
+    float head[MA], raw[MA];
 #pragma unroll
-    for (int j = 0; j < MAXA; ++j) head[j] = (j < AH) ? sB[j] : 0.f;
+    for (int j = 0; j < MA; ++j) {
+        head[j] = (j < AH) ? sB[j] : 0.f;
+        if (SD) raw[j] = (j < A) ? sB[AH + j] : 0.f;
+    }
     const float* row = tile + tid * (Hl + 1);
     for (int k = 0; k < Hl; ++k) {
         const float a = row[k];
 #pragma unroll
-        for (int j = 0; j < MAXA; ++j)
+        for (int j = 0; j < MA; ++j) {
             if (j < AH) head[j] = fmaf(a, sW[j * Hl + k], head[j]);
+            if (SD && !values_only && j < A) raw[j] = fmaf(a, sW[(AH + j) * Hl + k], raw[j]);
+        }
     }
     // value: denorm_value (running_mean_std.py:104-106): sqrt(var+eps)*clamp(v,-5,5)+mean
     float val = head[0];
@@ -59,14 +69,14 @@ __global__ void __launch_bounds__(PT) policy_head_sample_kernel(
     values[e] = val;
     if (values_only) return;
     // noise
-    float eps[MAXA];
+    float eps[MA];
     if (noise) {
 #pragma unroll
-        for (int j = 0; j < MAXA; ++j) eps[j] = (j < A) ? __ldg(noise + (int64_t)e * A + j) : 0.f;
+        for (int j = 0; j < MA; ++j) eps[j] = (j < A) ? __ldg(noise + (int64_t)e * A + j) : 0.f;
     } else {
         const uint64_t ep = rng_epoch_dev ? *rng_epoch_dev : 0ull;
 #pragma unroll
-        for (int q = 0; q < MAXA / 4; ++q) {
+        for (int q = 0; q < MA / 4; ++q) {
             if (q * 4 < A) {
                 const Philox4 r = philox4x32_10((uint64_t)e, (ep << 20) | ((uint64_t)step_index << 4) | (uint64_t)q, seed);
                 box_muller(r.x, r.y, eps[q * 4 + 0], eps[q * 4 + 1]);
@@ -76,13 +86,15 @@ __global__ void __launch_bounds__(PT) policy_head_sample_kernel(
     }
     float sumz2 = 0.f, sumls = 0.f;
 #pragma unroll
-    for (int j = 0; j < MAXA; ++j) {
+    for (int j = 0; j < MA; ++j) {
         if (j < A) {
-            const float mu = head[1 + j], sg = sSig[j];
+            float sg_sd = 0.f, ls_sd = 0.f, unused;
+            if (SD) sigma_param(raw[j], scfg, sg_sd, ls_sd, unused);
+            const float mu = head[1 + j], sg = SD ? sg_sd : sSig[j];
             const float act = __fadd_rn(mu, __fmul_rn(sg, eps[j]));
             const float z = (act - mu) / sg;
             sumz2 += z * z;
-            sumls += sSig[A + j];
+            sumls += SD ? ls_sd : sSig[A + j];
             actions[(int64_t)e * A + j] = act;
             mus[(int64_t)e * A + j] = mu;
             sigmas[(int64_t)e * A + j] = sg;
@@ -100,6 +112,35 @@ __global__ void __launch_bounds__(PT) policy_head_sample_kernel(
     neglogp[e] = 0.5f * sumz2 + 0.9189385332046727f * (float)A + sumls;
     if (dones_out) dones_out[e] = dones_cur[e];
     if (valid_out) valid_out[e] = prev_dones ? (1.0f - prev_dones[e]) : 1.0f;
+}
+
+__global__ void __launch_bounds__(PT) policy_head_sample_kernel(
+    const float* __restrict__ a_last, int Hl, const float* __restrict__ Wh, const float* __restrict__ bh,
+    const float* __restrict__ logstd, const double* __restrict__ vms_mean, const double* __restrict__ vms_var,
+    int normalize_value, const float* __restrict__ noise, uint64_t seed, const uint64_t* __restrict__ rng_epoch_dev,
+    uint32_t step_index, float* __restrict__ actions, float* __restrict__ mus, float* __restrict__ sigmas,
+    float* __restrict__ neglogp, float* __restrict__ values, float* __restrict__ env_actions, int clip_actions,
+    const float* __restrict__ act_low, const float* __restrict__ act_high,
+    const uint8_t* __restrict__ dones_cur, uint8_t* __restrict__ dones_out, const float* __restrict__ prev_dones,
+    float* __restrict__ valid_out, int N, int A, int values_only) {
+    policy_head_sample_body<MAXA, false>(a_last, Hl, Wh, bh, logstd, vms_mean, vms_var, normalize_value, noise, seed, rng_epoch_dev,
+                                         step_index, actions, mus, sigmas, neglogp, values, env_actions, clip_actions, act_low, act_high,
+                                         dones_cur, dones_out, prev_dones, valid_out, N, A, values_only, SigmaCfgDev{});
+}
+
+// state-dependent sigma (A <= 15)
+__global__ void __launch_bounds__(PT) policy_head_sample_sd_kernel(
+    const float* __restrict__ a_last, int Hl, const float* __restrict__ Wh, const float* __restrict__ bh,
+    SigmaCfgDev scfg, const double* __restrict__ vms_mean, const double* __restrict__ vms_var,
+    int normalize_value, const float* __restrict__ noise, uint64_t seed, const uint64_t* __restrict__ rng_epoch_dev,
+    uint32_t step_index, float* __restrict__ actions, float* __restrict__ mus, float* __restrict__ sigmas,
+    float* __restrict__ neglogp, float* __restrict__ values, float* __restrict__ env_actions, int clip_actions,
+    const float* __restrict__ act_low, const float* __restrict__ act_high,
+    const uint8_t* __restrict__ dones_cur, uint8_t* __restrict__ dones_out, const float* __restrict__ prev_dones,
+    float* __restrict__ valid_out, int N, int A, int values_only) {
+    policy_head_sample_body<MAXA_SD, true>(a_last, Hl, Wh, bh, nullptr, vms_mean, vms_var, normalize_value, noise, seed, rng_epoch_dev,
+                                           step_index, actions, mus, sigmas, neglogp, values, env_actions, clip_actions, act_low, act_high,
+                                           dones_cur, dones_out, prev_dones, valid_out, N, A, values_only, scfg);
 }
 
 struct ShaperDev {
@@ -244,6 +285,35 @@ B200RL_EXPORT int b200rl_policy_head_sample_f32(const float* a_last, int Hl, con
         a_last, Hl, W_head, b_head, logstd, vms_mean, vms_var, normalize_value, noise, seed, rng_epoch_dev, step_index, actions, mus,
         sigmas, neglogp, values, env_actions, clip_actions, act_low, act_high, dones_cur, dones_out, prev_dones, valid_out, N, A,
         values_only);
+    B200RL_LAUNCH_CHECK();
+    return B200RL_OK;
+}
+
+B200RL_EXPORT int b200rl_policy_head_sample_sd_f32(const float* a_last, int Hl, const float* W_head, const float* b_head,
+                                                   const b200rl_sigma_cfg* sigma_cfg_host, const double* vms_mean, const double* vms_var,
+                                                   int normalize_value, const float* noise, uint64_t seed,
+                                                   const uint64_t* rng_epoch_dev, uint32_t step_index,
+                                                   float* actions, float* mus, float* sigmas, float* neglogp, float* values,
+                                                   float* env_actions, int clip_actions, const float* act_low, const float* act_high,
+                                                   const uint8_t* dones_cur, uint8_t* dones_out, const float* prev_dones,
+                                                   float* valid_out, int N, int A, int values_only, void* stream) {
+    if (!a_last || !W_head || !b_head || !sigma_cfg_host || !values || N <= 0 || A <= 0 || A + 1 > MAXA_SD || Hl <= 0) return B200RL_EINVAL;
+    if (sigma_cfg_host->parametrization < SIGMA_EXP || sigma_cfg_host->parametrization > SIGMA_LINEAR) return B200RL_EINVAL;
+    if (!values_only && (!actions || !mus || !sigmas || !neglogp)) return B200RL_EINVAL;
+    if (normalize_value && (!vms_mean || !vms_var)) return B200RL_EINVAL;
+    if (env_actions && clip_actions && (!act_low || !act_high)) return B200RL_EINVAL;
+    if (dones_out && !dones_cur) return B200RL_EINVAL;
+    const int HR = 1 + 2 * A;
+    const size_t smem = sizeof(float) * ((size_t)PT * (Hl + 1) + (size_t)HR * Hl + HR + 2 * A);
+    if (smem > 200 * 1024) return B200RL_EUNSUPPORTED;
+    if (smem > 48 * 1024) {
+        cudaError_t e = cudaFuncSetAttribute(policy_head_sample_sd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return (int)e;
+    }
+    policy_head_sample_sd_kernel<<<(N + PT - 1) / PT, PT, smem, as_stream(stream)>>>(
+        a_last, Hl, W_head, b_head, sigma_cfg_dev(*sigma_cfg_host), vms_mean, vms_var, normalize_value, noise, seed, rng_epoch_dev,
+        step_index, actions, mus, sigmas, neglogp, values, env_actions, clip_actions, act_low, act_high, dones_cur, dones_out, prev_dones,
+        valid_out, N, A, values_only);
     B200RL_LAUNCH_CHECK();
     return B200RL_OK;
 }

@@ -2,13 +2,17 @@
 
 Mirrors the call surface of the reference's ``ModelA2CContinuousLogStd.Network`` (models.py:304-364)
 wrapped around ``A2CBuilder.Network`` (network_builder.py:211-593) for the subset on the hot path:
-shared MLP trunk (``separate: False``), ``fixed_sigma: True`` continuous head with the 'exp' sigma
-parametrisation, scalar value head, optional obs / value ``RunningMeanStd`` normalisers.
+MLP trunk, continuous head with a fixed (``fixed_sigma: True``) or state-dependent (``fixed_sigma: False``) sigma in any of the
+reference's sigma parametrisations, scalar value head, optional obs / value ``RunningMeanStd`` normalisers.
 
 All parameters live in ONE flat fp32 arena (``self.flat``) with matching flat gradient / Adam-moment
 arenas, so the optimiser, the gradient all-reduce and the checkpoint code each touch one buffer:
 
     [ sigma(A) | W_1 | b_1 | ... | W_L | b_L | W_head(A+1, H_L) | b_head(A+1) ]   (row 0 of the head = value)
+
+A state-dependent sigma head (``fixed_sigma: False``) is A more head rows, ``W_head(1+2A, H_L) | b_head(1+2A)`` = (value, mu, sigma);
+the leading ``sigma(A)`` block then stays in the arena as dead space that is always exactly zero (no state-dict key, no Adam state,
+no gradient), so every offset convention of the fixed-sigma layout holds for both.
 
 ``state_dict()`` / ``load_state_dict()`` speak the reference's key names
 (``a2c_network.sigma``, ``a2c_network.actor_mlp.{0,2,..}.{weight,bias}``, ``a2c_network.value.*``,
@@ -115,7 +119,7 @@ class _NetworkView:
 
     def __init__(self, model):
         self._m = model
-        self.fixed_sigma = True
+        self.fixed_sigma = model.fixed_sigma
 
     @property
     def sigma(self):
@@ -284,15 +288,28 @@ class B200Model(FlatParamModel):
         # default) = obs -> MLP -> LSTM -> heads.  Same parameter names and order either way, different shapes.
         self.rnn_before_mlp = bool(network_params.get('rnn', {}).get('before_mlp', False)) if self.rnn_units else True
         space = network_params['space']['continuous']
-        if not space.get('fixed_sigma', True):
-            raise NotImplementedError('state-dependent sigma is not on the B200 hot path yet')
+        # fixed_sigma: False (network_builder.py:324-348, :441-444): sigma = Linear(H_L, A) of the trunk output, one std per row
+        self.fixed_sigma = bool(space.get('fixed_sigma', True))
+        if not self.fixed_sigma:
+            if self.separate:
+                raise NotImplementedError('state-dependent sigma with separate actor/critic trunks is not on the B200 hot path')
+            if 'rnn' in network_params:
+                raise NotImplementedError('state-dependent sigma with an rnn is not on the B200 hot path')
         for k in ('mu_activation', 'sigma_activation'):
             if space.get(k, 'None') not in ('None', None):
                 raise NotImplementedError(f'{k}={space[k]}')
-        if space.get('sigma_parametrization', 'exp') != 'exp' or space.get('logstd_bounds'):
-            raise NotImplementedError("only the 'exp' sigma parametrisation (optionally floored by min_sigma) is on the B200 hot path")
-        # models.py:272-300, 'exp' branch with a floor (configs/mjlab/ppo_lift_cube_yam.yaml: min_sigma 0.15): sigma = exp(raw) + min_sigma
+        # models.py:272-302 apply_sigma_parametrization: 'exp' (clamped to logstd_bounds, floored by min_sigma), 'softplus', 'linear'
+        # (alias 'scalar'); configs/mjlab/ppo_lift_cube_yam.yaml: exp + min_sigma 0.15, ppo_wujihand_reorient.yaml: softplus + 0.2
+        self.sigma_parametrization = space.get('sigma_parametrization', 'exp')
+        if self.sigma_parametrization not in ops.SIGMA_PARAM:
+            raise NotImplementedError(f'sigma_parametrization {self.sigma_parametrization}')
         self.min_sigma = float(space.get('min_sigma', 0.0) or 0.0)
+        bounds = space.get('logstd_bounds', None)
+        self.logstd_bounds = (float(bounds[0]), float(bounds[1])) if bounds is not None and self.sigma_parametrization == 'exp' else None
+        self.sigma_cfg = ops.sigma_cfg(self.sigma_parametrization, self.min_sigma, self.logstd_bounds)
+        # a fixed sigma that is not the plain log-std is mapped outside the kernels (refresh_sigma_floor)
+        self.sigma_transform = self.fixed_sigma and (self.sigma_parametrization != 'exp' or self.min_sigma > 0 or self.logstd_bounds is not None)
+        self.head_rows = int(act_dim) + 1 if self.fixed_sigma else 1 + 2 * int(act_dim)      # (value, mu[, sigma]) rows of W_head
         if network_params.get('value_activation', 'None') not in ('None', None):
             raise NotImplementedError('value_activation')
         self.D, self.A = int(obs_dim), int(act_dim)
@@ -311,7 +328,7 @@ class B200Model(FlatParamModel):
         if Hd and not self.rnn_before_mlp:
             ins = Hd                     # the heads read the LSTM output
         self.Hl = ins
-        sizes += [('W_head', (self.A + 1, ins)), ('b_head', (self.A + 1,))]
+        sizes += [('W_head', (self.head_rows, ins)), ('b_head', (self.head_rows,))]
         # every tensor starts on an 8-element boundary (32 bytes in the fp32 arenas, 16 bytes in the bf16 twin the tensor-core GEMMs
         # read): weight rows can then be staged with 16-byte loads whatever the action count did to the offsets.  The gaps hold
         # zeros in every arena (weights, gradients, moments), so norms, Adam and the all-reduce are unaffected; layouts whose tensor
@@ -322,7 +339,7 @@ class B200Model(FlatParamModel):
         self.W = [self.view(f'W{i}') for i in range(len(self.units))]
         self.b = [self.view(f'b{i}') for i in range(len(self.units))]
         self.sigma = self.view('sigma')
-        if self.min_sigma > 0:
+        if self.sigma_transform:
             # what the kernels are handed instead of the raw parameter, and the chain factor of its gradient (refresh_sigma_floor)
             self.logstd_eff = torch.zeros(self.A, dtype=torch.float32, device=self.device)
             self.sigma_chain = torch.ones(self.A, dtype=torch.float32, device=self.device)
@@ -348,21 +365,46 @@ class B200Model(FlatParamModel):
     # -------------------------------------------------------------------------------------------
     @property
     def logstd_in(self):
-        """The log-std vector the policy kernels read.  They compute sigma = exp(logstd) -- with a floor (min_sigma > 0) that is the
-        EFFECTIVE log-std log(exp(raw) + min_sigma) (models.py:296-300: `sigma + min_sigma`, `logstd = log(sigma)`), kept in its own
-        buffer by refresh_sigma_floor(); without a floor it is the parameter itself."""
-        return self.logstd_eff if self.min_sigma > 0 else self.sigma
+        """The log-std vector the fixed-sigma policy kernels read.  They compute sigma = exp(logstd) -- for any sigma other than the
+        plain log-std (a floor, bounds, 'softplus' / 'linear') that is the EFFECTIVE log-std log(sigma(raw)) (models.py:272-302), kept
+        in its own buffer by refresh_sigma_floor(); otherwise it is the parameter itself."""
+        return self.logstd_eff if self.sigma_transform else self.sigma
 
     def refresh_sigma_floor(self):
-        """After anything that changes the raw sigma parameter (optimiser step, weight load): logstd_eff = log(e^raw + min_sigma) and
-        sigma_chain = d logstd_eff / d raw = e^raw / (e^raw + min_sigma), the factor that turns the kernels' gradient with respect to
-        the log-std they were handed into the gradient of the raw parameter.  Three in-place launches on [A] vectors, no allocation
-        (CUDA-graph capturable); a no-op without a floor."""
-        if self.min_sigma > 0:
+        """After anything that changes the raw fixed sigma parameter (optimiser step, weight load): logstd_eff = log(sigma(raw)) and
+        sigma_chain = d logstd_eff / d raw, the factor that turns the kernels' gradient with respect to the log-std they were handed
+        into the gradient of the raw parameter.  In-place launches on [A] vectors (CUDA-graph capturable); a no-op for the plain
+        log-std and for a state-dependent head, whose kernels apply the parametrisation per row."""
+        if not self.sigma_transform:
+            return
+        if self.sigma_parametrization == 'exp' and self.logstd_bounds is None:     # exp(raw) + min_sigma
             torch.exp(self.sigma, out=self.sigma_chain)
             torch.add(self.sigma_chain, self.min_sigma, out=self.logstd_eff)
             self.sigma_chain.div_(self.logstd_eff)
             self.logstd_eff.log_()
+            return
+        raw = self.sigma
+        if self.sigma_parametrization == 'exp':
+            lo, hi = self.logstd_bounds
+            g = ((raw >= lo) & (raw <= hi)).float()             # torch.clamp's gradient: 1 on the closed interval
+            rc = raw.clamp(lo, hi)
+            if self.min_sigma > 0:
+                e = rc.exp()
+                torch.add(e, self.min_sigma, out=self.logstd_eff)
+                torch.mul(e, g, out=self.sigma_chain)
+                self.sigma_chain.div_(self.logstd_eff)
+                self.logstd_eff.log_()
+            else:
+                self.logstd_eff.copy_(rc)
+                self.sigma_chain.copy_(g)
+            return
+        floor_ = max(self.min_sigma, 1e-3) if self.sigma_parametrization in ('linear', 'scalar') else self.min_sigma
+        x = raw - floor_ if self.sigma_parametrization in ('linear', 'scalar') else raw
+        torch.add(torch.nn.functional.softplus(x), floor_, out=self.logstd_eff)        # sigma
+        z = x.exp()
+        torch.where(x > 20.0, torch.ones_like(x), z / (z + 1.0), out=self.sigma_chain)  # softplus' (threshold 20)
+        self.sigma_chain.div_(self.logstd_eff)
+        self.logstd_eff.log_()
 
     def _init_weights(self, network_params, seed):
         """network_builder.py:326-348: mlp initializer on every Linear weight, zero biases, mu_init on mu.weight,
@@ -392,15 +434,28 @@ class B200Model(FlatParamModel):
                 cpu[f'W{i}'] = w
                 ins = u
             ins = self.Hl
-            wh = torch.empty(self.A + 1, ins)
+            A = self.A
+            wh = torch.empty(self.head_rows, ins)
             _apply_init(wh[:1], mlp_init, ins)                                   # value head: mlp_init
-            _apply_init(wh[1:], mlp_init, ins)
+            _apply_init(wh[1:A + 1], mlp_init, ins)
             if mu_init.get('name', 'default') != 'default':
-                _apply_init(wh[1:], mu_init, ins)
+                _apply_init(wh[1:A + 1], mu_init, ins)
+            sigma_init = space.get('sigma_init', {'name': 'const_initializer', 'val': 0})
+            if not self.fixed_sigma:
+                # network_builder.py:14-25 init_state_dependent_sigma_head, after the mlp_init pass over every Linear: a const
+                # initializer writes the bias and zeroes the weight, anything else initialises the weight (bias stays zero)
+                _apply_init(wh[A + 1:], mlp_init, ins)
+                if sigma_init.get('name') == 'const_initializer':
+                    wh[A + 1:].zero_()
+                    cpu['b_head'] = torch.zeros(self.head_rows)
+                    cpu['b_head'][A + 1:] = float(sigma_init.get('val', 0.0))
+                else:
+                    _apply_init(wh[A + 1:], sigma_init, ins)
             cpu['W_head'] = wh
-        sg = torch.empty(self.A)
-        _apply_init(sg, space.get('sigma_init', {'name': 'const_initializer', 'val': 0}), 1)
-        cpu['sigma'] = sg
+        if self.fixed_sigma:
+            sg = torch.empty(self.A)
+            _apply_init(sg, space.get('sigma_init', {'name': 'const_initializer', 'val': 0}), 1)
+            cpu['sigma'] = sg
         for n, t in cpu.items():
             self.view(n).copy_(t)
 
@@ -429,7 +484,8 @@ class B200Model(FlatParamModel):
         return self
 
     def parameters(self):
-        """Reference parameter order (optimizer state is index-keyed): sigma, actor_mlp.*, value.*, mu.*"""
+        """Reference parameter order (optimizer state is index-keyed): sigma, actor_mlp.*, value.*, mu.* (state-dependent head:
+        actor_mlp.*, value.*, mu.*, sigma.weight, sigma.bias)"""
         return self._param_views(self.flat)
 
     def _param_views(self, arena=None):
@@ -441,7 +497,10 @@ class B200Model(FlatParamModel):
         if self.rnn_units:   # registration order in A2CBuilder.Network.__init__: actor_mlp placeholder precedes self.rnn
             out += [self.view(n, arena) for n in ('W_ih', 'W_hh', 'b_ih', 'b_hh')]
         wh, bh = self.view('W_head', arena), self.view('b_head', arena)
-        out += [wh[:1], bh[:1], wh[1:], bh[1:]]
+        A = self.A
+        out += [wh[:1], bh[:1], wh[1:A + 1], bh[1:A + 1]]
+        if not self.fixed_sigma:        # a Linear sigma head is registered after mu; the leading sigma block is dead space
+            out = out[1:] + [wh[A + 1:], bh[A + 1:]]
         return out
 
     def _param_views_separate(self, arena):
@@ -460,7 +519,12 @@ class B200Model(FlatParamModel):
         return out
 
     def param_names(self):
-        """state-dict keys of _param_views, in the same order: sigma, actor_mlp.*, [critic_mlp.*], [rnn.*], value.*, mu.*"""
+        """state-dict keys of _param_views, in the same order: sigma, actor_mlp.*, [critic_mlp.*], [rnn.*], value.*, mu.*; a
+        state-dependent head: actor_mlp.*, value.*, mu.*, sigma.weight, sigma.bias"""
+        if not self.fixed_sigma:
+            keys = [f'a2c_network.actor_mlp.{2 * i}.{t}' for i in range(len(self.trunk_units)) for t in ('weight', 'bias')]
+            return keys + ['a2c_network.value.weight', 'a2c_network.value.bias', 'a2c_network.mu.weight', 'a2c_network.mu.bias',
+                           'a2c_network.sigma.weight', 'a2c_network.sigma.bias']
         keys = ['a2c_network.sigma']
         for trunk in (('actor_mlp', 'critic_mlp') if self.separate else ('actor_mlp',)):
             for i in range(len(self.trunk_units)):

@@ -20,6 +20,21 @@ class LossCfg(ctypes.Structure):
                 ('use_smooth_clamp', ctypes.c_int), ('ppo', ctypes.c_int)]
 
 
+class SigmaCfg(ctypes.Structure):
+    """b200rl_sigma_cfg: the sigma parametrisation of a policy (models.py apply_sigma_parametrization)"""
+    _fields_ = [('parametrization', ctypes.c_int), ('min_sigma', ctypes.c_float), ('has_logstd_bounds', ctypes.c_int),
+                ('logstd_lo', ctypes.c_float), ('logstd_hi', ctypes.c_float)]
+
+
+# sigma_parametrization names -> b200rl_sigma_cfg.parametrization ('scalar' is the reference's alias of 'linear')
+SIGMA_PARAM = {'exp': 0, 'softplus': 1, 'linear': 2, 'scalar': 2}
+
+
+def sigma_cfg(parametrization='exp', min_sigma=0.0, logstd_bounds=None):
+    lo, hi = (float(logstd_bounds[0]), float(logstd_bounds[1])) if logstd_bounds is not None else (0.0, 0.0)
+    return SigmaCfg(SIGMA_PARAM[parametrization], float(min_sigma), int(logstd_bounds is not None), lo, hi)
+
+
 class OptCfg(ctypes.Structure):
     _fields_ = [('beta1', ctypes.c_double), ('beta2', ctypes.c_double), ('eps', ctypes.c_double),
                 ('weight_decay', ctypes.c_double), ('grad_norm', ctypes.c_double), ('kl_threshold', ctypes.c_double),
@@ -233,6 +248,21 @@ def ppo_head_loss(a_last, W_head, b_head, logstd, actions, old_mu, old_sigma, ol
     return nb.value
 
 
+def ppo_head_loss_sd(a_last, W_head, b_head, sigma_cfg, entropy_coef_dev, actions, old_mu, old_sigma, old_values_n, returns_n,
+                     old_neglogp, advs_n, mask, rows_per_chunk, chunk_stride, M, A, cfg, inv_count, d_head, d_alast, act_last, partials,
+                     mu_out=None, value_out=None, neglogp_out=None):
+    """ppo_head_loss for a state-dependent sigma head: W_head [1 + 2A, Hl] (value, mu, raw sigma), d_head [M, 1 + 2A]"""
+    nb = ctypes.c_int(0)
+    Hl = W_head.shape[1]
+    check(lib.b200rl_ppo_head_loss_sd_f32(ptr(a_last), Hl, ptr(W_head), ptr(b_head), ctypes.addressof(sigma_cfg), ptr(entropy_coef_dev),
+                                          ptr(actions), ptr(old_mu), ptr(old_sigma), ptr(old_values_n), ptr(returns_n), ptr(old_neglogp),
+                                          ptr(advs_n), ptr(mask), rows_per_chunk, chunk_stride, M, A, ctypes.addressof(cfg),
+                                          ptr(inv_count), ptr(d_head), ptr(d_alast), act_last, ptr(mu_out), ptr(value_out),
+                                          ptr(neglogp_out), ptr(partials), partials.shape[0], ctypes.addressof(nb),
+                                          _stream()), 'ppo_head_loss_sd')
+    return nb.value
+
+
 def ppo_loss_finalize(partials, n_partials, A, entropy_coef_dev, stats, d_logstd, kl_out=None):
     check(lib.b200rl_ppo_loss_finalize(ptr(partials), n_partials, A, ptr(entropy_coef_dev), ptr(stats), ptr(d_logstd),
                                        ptr(kl_out), _stream()), 'ppo_loss_finalize')
@@ -303,6 +333,19 @@ def policy_head_sample(a_last, W_head, b_head, logstd, vms_mean, vms_var, normal
                                             ptr(env_actions), int(clip_actions), ptr(act_low), ptr(act_high),
                                             ptr(dones_cur), ptr(dones_out), ptr(prev_dones), ptr(valid_out), N, A,
                                             int(values_only), _stream()), 'policy_head_sample')
+
+
+def policy_head_sample_sd(a_last, W_head, b_head, sigma_cfg, vms_mean, vms_var, normalize_value, noise, seed, rng_epoch,
+                          step_index, actions, mus, sigmas, neglogp, values, env_actions, clip_actions, act_low, act_high,
+                          dones_cur, dones_out, prev_dones, valid_out, N, A, values_only=False):
+    """policy_head_sample for a state-dependent sigma head: W_head [1 + 2A, Hl] (value, mu, raw sigma), sigma per row"""
+    Hl = W_head.shape[1]
+    check(lib.b200rl_policy_head_sample_sd_f32(ptr(a_last), Hl, ptr(W_head), ptr(b_head), ctypes.addressof(sigma_cfg), ptr(vms_mean),
+                                               ptr(vms_var), int(normalize_value), ptr(noise), seed, ptr(rng_epoch),
+                                               step_index, ptr(actions), ptr(mus), ptr(sigmas), ptr(neglogp), ptr(values),
+                                               ptr(env_actions), int(clip_actions), ptr(act_low), ptr(act_high),
+                                               ptr(dones_cur), ptr(dones_out), ptr(prev_dones), ptr(valid_out), N, A,
+                                               int(values_only), _stream()), 'policy_head_sample_sd')
 
 
 def post_step(rewards, dones, time_outs, values_t, valid_t, rewards_out_t, dones_cur, prev_dones, ep_state, meter,
