@@ -99,6 +99,18 @@ int b200rl_adv_ema_normalize_f32(float* advs, int B, const double* partials, int
 int b200rl_batch_moments_f64(const float* values, const float* returns, const float* mask, double* partials,
                              int max_partials, int B, int* n_blocks_out_host, void* stream);
 
+/* Explained variance of every minibatch (torch_ext.explained_variance, torch_ext.py:204-215) for the `use_diagnostics` summaries:
+ * minibatch i = n_chunks chunks of rows_per_chunk rows, chunk c starting at row i*mb_offset + c*chunk_stride of values / returns
+ * (the normalised old values and returns of the arena, [H, N] time-major: rows_per_chunk = envs per minibatch, n_chunks = H,
+ * chunk_stride = N, mb_offset = envs per minibatch; an LSTM minibatch's BPTT windows cover the same rows).  mask (nullable): rows
+ * with mask == 0 are left out.  Unmasked: 1 - var(r - v) / var(r), population variances; masked: 1 - var_m(r - v) / var_m(v) with
+ * get_mean_var_with_masks' clamped, Bessel-corrected variances.  fp64 sums, one block per minibatch, no atomics.  The value of
+ * minibatch i is written to out[i*out_stride + k*rep_stride] for k < n_rep (e.g. column B200RL_STAT_EXPVAR of the stats row of
+ * every mini-epoch's update of that minibatch). */
+int b200rl_explained_variance_f32(const float* values, const float* returns, const float* mask, int rows_per_chunk, int n_chunks,
+                                  int64_t chunk_stride, int n_mb, int64_t mb_offset, float* out, int64_t out_stride, int n_rep,
+                                  int64_t rep_stride, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * RunningMeanStd (running_mean_std.py:19-114) as standalone ops.
  * x: [R, D] rows given as n_chunks chunks of rows_per_chunk rows, chunk c starting at row c*chunk_stride.
@@ -211,6 +223,7 @@ typedef struct b200rl_loss_cfg {
 #define B200RL_STAT_CLIPFRAC 6
 #define B200RL_STAT_LR 7      /* lr used for this minibatch's Adam step (written by adam) */
 #define B200RL_STAT_GNORM 8   /* global grad norm before clipping (written by adam) */
+#define B200RL_STAT_EXPVAR 9  /* explained variance of the minibatch (b200rl_explained_variance_f32, use_diagnostics only) */
 #define B200RL_NSTATS 16
 
 /* Head GEMM + loss forward + backward down to d(a_last).

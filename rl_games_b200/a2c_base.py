@@ -14,6 +14,7 @@ import torch.distributed as dist
 
 from .common import (AdaptiveScheduler, IdentityScheduler, LinearScheduler, DefaultAlgoObserver, DefaultRewardsShaper,
                      create_vec_env, make_summary_writer)
+from .diagnostics import PpoDiagnostics, make_diagnostics, replay as replay_diagnostics
 from .dist_utils import PackedStatsSync
 from .model import CompileTolerantModel, resolve_device
 
@@ -109,6 +110,10 @@ class A2CBase(CompileTolerantModel):
         rs = config['reward_shaper']
         self.rewards_shaper = rs if not isinstance(rs, dict) else DefaultRewardsShaper(**rs)
         self.mini_epochs_num = config['mini_epochs']
+        # a2c_common.py:222-227: PPO diagnostics summaries on rank 0; the device work they need runs only where this is True
+        self.use_diagnostics = bool(config.get('use_diagnostics', False))
+        self.diagnostics = make_diagnostics(self.use_diagnostics, self.global_rank)
+        self.diag_on = isinstance(self.diagnostics, PpoDiagnostics)
         self.last_lr = float(config['learning_rate'])
         self.is_adaptive_lr = config['lr_schedule'] == 'adaptive'
         self.linear_lr = config['lr_schedule'] == 'linear'
@@ -268,6 +273,7 @@ class A2CBase(CompileTolerantModel):
             frame = self.frame // self.num_agents
             should_exit = False
             if self.global_rank == 0:
+                self.diagnostics.epoch(self, current_epoch=epoch_num)
                 if self.print_stats:
                     st = max(step_time, 1e-9)
                     print(f'fps step: {curr_frames / st:.0f} fps step and policy inference: {curr_frames / play_time:.0f} '
@@ -333,6 +339,7 @@ class A2CBase(CompileTolerantModel):
                     last_lr, lr_mul, frame, scaled_time, scaled_play_time, curr_frames):
         """a2c_common.py:527-547: the same summary scalars, tag for tag"""
         w = self.writer
+        self.diagnostics.send_info(w)
         w.add_scalar('performance/step_inference_rl_update_fps', curr_frames / scaled_time, frame)
         w.add_scalar('performance/step_inference_fps', curr_frames / scaled_play_time, frame)
         w.add_scalar('performance/step_fps', curr_frames / max(step_time, 1e-9), frame)
@@ -349,6 +356,37 @@ class A2CBase(CompileTolerantModel):
         w.add_scalar('info/kl', kl, frame)
         w.add_scalar('info/epochs', epoch_num, frame)
         self.algo_observer.after_print_stats(frame, epoch_num, total_time)
+
+    # =============================================================================== PPO diagnostics (use_diagnostics)
+    def _replay_diagnostics(self, exp_var, clip_frac, sum_mask):
+        """one epoch's per-update host columns -> diagnostics.mini_batch / mini_epoch in update order"""
+        replay_diagnostics(self, exp_var, clip_frac, sum_mask, self.mask_autoreset_rows, self.minibatch_size, self.num_minibatches,
+                           self.mini_epochs_num, self.e_clip)
+
+    def diagnostics_normaliser_stats(self):
+        """diagnostics/rms_* values of the last epoch's read-back (PpoDiagnostics.epoch, diagnostics.py:30-41)"""
+        out = {}
+        if getattr(self, 'normalize_rms_advantage', False):
+            mean, sqrs = self._diag_adv_host[0:1].clone(), self._diag_adv_host[1:2].clone()
+            std = torch.sqrt(torch.clamp_min(sqrs - mean.pow(2), 1 / 1e5 ** 2))      # GeneralizedMovingStats max = 1e5, eps = 0
+            out['diagnostics/rms_advantage/mean'] = float(mean)
+            out['diagnostics/rms_advantage/var'] = float(std * std)
+        if self.normalize_value:
+            out['diagnostics/rms_value/mean'] = float(self._diag_vms_host[0])
+            out['diagnostics/rms_value/var'] = float(self._diag_vms_host[1])
+        return out
+
+    def _diag_readback(self):
+        """queues the D2H copies of the normaliser statistics behind the epoch (the caller's one synchronise covers them)"""
+        if not hasattr(self, '_diag_vms_host'):
+            self._diag_vms_host = torch.zeros(2, dtype=torch.float64).pin_memory()
+            self._diag_adv_host = torch.zeros(2, dtype=torch.float32).pin_memory()
+        vms = self.value_mean_std
+        if self.normalize_value and vms is not None:
+            self._diag_vms_host[0:1].copy_(vms.running_mean.reshape(-1)[:1], non_blocking=True)
+            self._diag_vms_host[1:2].copy_(vms.running_var.reshape(-1)[:1], non_blocking=True)
+        if getattr(self, 'normalize_rms_advantage', False):
+            self._diag_adv_host.copy_(self.adv_ema_state, non_blocking=True)
 
     # =============================================================================== weights / checkpoints (a2c_common.py:825-921)
     def get_weights(self):

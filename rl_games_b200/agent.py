@@ -689,6 +689,10 @@ class A2CAgent(A2CBase):
                                   self.adv_rms_momentum, training=True)
         if self.mask_autoreset_rows:
             ops.mask_inv_counts(self.valid, self.horizon_length, self.num_actors, self.envs_per_mb, self.inv_counts)
+        if self.diag_on:
+            # diagnostics/exp_var of every minibatch from the prepared dataset, into column B200RL_STAT_EXPVAR of each of its updates' rows
+            ops.explained_variance(self.old_values_n, self.returns_n, self.valid, self.horizon_length, self.num_actors, self.envs_per_mb,
+                                   self.stats[:, ops.STAT_EXPVAR], n_rep=self.mini_epochs_num)
         if self.use_mb_moments:
             # obs are fixed for the whole update phase: batch sums of every minibatch in ONE pass over the arena
             ops.obs_mb_moments(self.obses, m.D, self.horizon_length, self.num_actors, self.envs_per_mb,
@@ -1031,6 +1035,8 @@ class A2CAgent(A2CBase):
         self.host_stats.copy_(self.stats, non_blocking=True)
         self.host_state[0:2].copy_(self.opt_state[0:2], non_blocking=True)
         self.host_state[2:10].copy_(self.meter, non_blocking=True)
+        if self.diag_on:
+            self._diag_readback()
         torch.cuda.current_stream().synchronize()
         self._meter_cache = self.host_state[2:10].numpy().copy()
         st = self.host_stats.clone()
@@ -1060,6 +1066,8 @@ class A2CAgent(A2CBase):
         nmb = self.num_minibatches
         kls = [st[e * nmb:(e + 1) * nmb, 4].mean() for e in range(self.mini_epochs_num)]
         self.last_stats = st
+        if self.diag_on:
+            self._replay_diagnostics(st[:, ops.STAT_EXPVAR], st[:, ops.STAT_CLIPFRAC], st[:, ops.STAT_SUMMASK])
         # the tuple's last_lr is what train_actor_critic returned for the LAST minibatch (a2c_common.py:1548, :1582): the lr that
         # minibatch ran on (stats column 7, written by the optimiser kernel), not self.last_lr after the final scheduler step
         return step_time, play_time, update_time, total_time, a_losses, c_losses, b_losses, entropies, kls, float(st[-1, 7]), 1.0

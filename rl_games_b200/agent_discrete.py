@@ -198,6 +198,8 @@ class DiscreteA2CAgent(A2CBase):
         self.n_splits = max(1, min(64, mb // 256))
         self.part = f(self.n_splits, m.num_params)
         self.grad = f(m.num_params)
+        self.diag_exp_var = f(self.num_minibatches) if self.diag_on else None
+        self._diag_clip = []
         self.loss_partials = torch.zeros((mb + 255) // 256, 8, dtype=torch.float64, device=dev)
         self.gae_partials = torch.zeros(max(64, (N + 63) // 64), 8, dtype=torch.float64, device=dev)
         self.inv_counts = f(self.num_minibatches) if self.mask_autoreset_rows else None
@@ -334,6 +336,9 @@ class DiscreteA2CAgent(A2CBase):
                           self.old_values_n, self.returns_n, self.advs_n, self.normalize_value, self.normalize_advantage)
         if self.mask_autoreset_rows:
             ops.mask_inv_counts(self.valid, self.horizon_length, self.num_actors, self.envs_per_mb, self.inv_counts)
+        if self.diag_on:        # diagnostics/exp_var of every minibatch from the prepared dataset
+            ops.explained_variance(self.old_values_n, self.returns_n, self.valid, self.horizon_length, self.num_actors, self.envs_per_mb,
+                                   self.diag_exp_var)
 
     # =============================================================================== update
     def _minibatch_update(self, i):
@@ -364,6 +369,8 @@ class DiscreteA2CAgent(A2CBase):
                                   None if self.inv_counts is None else self.inv_counts[i:i + 1], d_lg, d_ld, d_vl, d_vld,
                                   self.loss_partials, head_sizes=self.head_sizes)
         stats = self.loss_partials[:nb, :4].sum(dim=0).float()
+        if self.diag_on:            # (sum mask, sum mask * clipped) of the minibatch: its clip fraction for diagnostics/clip_frac
+            self._diag_clip.append(self.loss_partials[:nb, 4:6].sum(dim=0))
         # ---- backward through the heads and the trunk(s): split partial gradients, then one reduction ----
         off_wh, _ = m.layout['W_head']
         off_bh, _ = m.layout['b_head']
@@ -422,6 +429,7 @@ class DiscreteA2CAgent(A2CBase):
         self.curr_frames = self.batch_size
         self.algo_observer.after_steps()
         rows, kls = [], []
+        self._diag_clip = []
         for _ in range(self.mini_epochs_num):
             lr_used = self.last_lr          # what train_actor_critic returns for the minibatches of this mini-epoch (:1265, :1289)
             ep = [self._minibatch_update(i) for i in range(self.num_minibatches)]
@@ -435,10 +443,20 @@ class DiscreteA2CAgent(A2CBase):
             self.opt_state[0] = self.last_lr                        # update_lr
             kls.append(av_kl)
         self.sync_running_stats()
+        if self.diag_on:
+            clip_host = torch.empty(len(self._diag_clip), 2, dtype=torch.float64).pin_memory()
+            ev_host = torch.empty(self.num_minibatches, dtype=torch.float32).pin_memory()
+            clip_host.copy_(torch.stack(self._diag_clip), non_blocking=True)
+            ev_host.copy_(self.diag_exp_var, non_blocking=True)
+            self._diag_readback()
         self._sync()
         t2 = time.perf_counter()
         st = torch.stack(rows)
         self.last_stats = st
+        if self.diag_on:
+            # the loss kernels' clip fraction, as the continuous path's finalisation writes B200RL_STAT_CLIPFRAC
+            clip = (clip_host[:, 1] / clip_host[:, 0].clamp(min=1.0)).float()
+            self._replay_diagnostics(ev_host.repeat(self.mini_epochs_num), clip, clip_host[:, 0])
         a_losses, c_losses, entropies = list(st[:, 0]), list(st[:, 1]), list(st[:, 2])
         return step_time, t1 - t0, t2 - t1, t2 - t0, a_losses, c_losses, entropies, kls, lr_used, 1.0
 

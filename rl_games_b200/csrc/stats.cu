@@ -402,7 +402,89 @@ __global__ void __launch_bounds__(256) normalize_kernel(const float* __restrict_
     }
 }
 
+// ---- explained variance of every minibatch (torch_ext.py:204-215, PpoDiagnostics.mini_batch, diagnostics.py:55-62) ----------------
+// one 1024-thread block per minibatch, two passes over its rows (sums, then squared deviations from the means) in fp64; masked rows are skipped,
+// so whatever they hold contributes nothing.  ev[] = {n, ss_y, ss_dy}: unmasked y = returns (population variances); masked y = the
+// VALUES (the reference's get_mean_var_with_masks(y_pred, ...)) with its clamp(min=1) guards and Bessel factor.  var_y = 0 gives
+// -inf / NaN, like the reference.
+__host__ __device__ inline float expvar_finalize(double n, double ss_y, double ss_dy, int masked) {
+    double var_y, var_dy;
+    if (masked) {
+        const double s = n > 1.0 ? n : 1.0;
+        const double bessel = s / (s - 1.0 > 1.0 ? s - 1.0 : 1.0);
+        var_y = ss_y / s * bessel;
+        var_dy = ss_dy / s * bessel;
+    } else {
+        var_y = ss_y / n;
+        var_dy = ss_dy / n;
+    }
+    return (float)(1.0 - var_dy / var_y);
+}
+
+template <bool MASKED>
+__global__ void __launch_bounds__(1024) explained_variance_kernel(const float* __restrict__ values, const float* __restrict__ returns,
+                                                                 const float* __restrict__ mask, int rows_per_chunk, int n_chunks,
+                                                                 int64_t chunk_stride, int64_t mb_offset, float* __restrict__ out,
+                                                                 int64_t out_stride, int n_rep, int64_t rep_stride) {
+    __shared__ double sm[32 * 3];
+    const int64_t base = (int64_t)blockIdx.x * mb_offset;
+    // pass 1: count, sum y, sum (returns - values); rows walked chunk by chunk, coalesced within a chunk
+    double acc[3] = {0, 0, 0};
+    for (int c = 0; c < n_chunks; ++c) {
+        const int64_t rc = base + c * chunk_stride;
+#pragma unroll 2
+        for (int e = threadIdx.x; e < rows_per_chunk; e += blockDim.x) {
+            if (MASKED && mask[rc + e] == 0.f) continue;
+            const float v = values[rc + e], ret = returns[rc + e];
+            acc[0] += 1.0; acc[1] += (double)(MASKED ? v : ret); acc[2] += (double)__fsub_rn(ret, v);
+        }
+    }
+    block_sum_d<3>(acc, sm);
+    const double n = acc[0];
+    const double my = n > 0.0 ? acc[1] / n : 0.0, md = n > 0.0 ? acc[2] / n : 0.0;
+    // pass 2: squared deviations (the minibatch's rows are L2-resident after pass 1)
+    double sq[2] = {0, 0};
+    for (int c = 0; c < n_chunks; ++c) {
+        const int64_t rc = base + c * chunk_stride;
+#pragma unroll 2
+        for (int e = threadIdx.x; e < rows_per_chunk; e += blockDim.x) {
+            if (MASKED && mask[rc + e] == 0.f) continue;
+            const float v = values[rc + e], ret = returns[rc + e];
+            const double y = (double)(MASKED ? v : ret) - my, d = (double)__fsub_rn(ret, v) - md;
+            sq[0] += y * y; sq[1] += d * d;
+        }
+    }
+    block_sum_d<2>(sq, sm);
+    if (threadIdx.x == 0) {
+        const float ev = expvar_finalize(n, sq[0], sq[1], MASKED);
+        for (int k = 0; k < n_rep; ++k) out[(int64_t)blockIdx.x * out_stride + k * rep_stride] = ev;
+    }
+}
+
 }  // namespace
+
+#ifdef B200RL_TEST_HOOKS   // test-only host entry point: compiled into tests/libb200rl_testhooks.so (csrc/build.py), not into the product library
+// the explained-variance finalisation (expvar_finalize) over host arrays of (n, ss_y, ss_dy) triples
+B200RL_EXPORT int b200rl_hosttest_expvar_finalize(const double* sums, int count, int masked, float* out) {
+    for (int i = 0; i < count; ++i) out[i] = expvar_finalize(sums[3 * i], sums[3 * i + 1], sums[3 * i + 2], masked);
+    return B200RL_OK;
+}
+#endif  // B200RL_TEST_HOOKS
+
+B200RL_EXPORT int b200rl_explained_variance_f32(const float* values, const float* returns, const float* mask, int rows_per_chunk,
+                                                int n_chunks, int64_t chunk_stride, int n_mb, int64_t mb_offset, float* out,
+                                                int64_t out_stride, int n_rep, int64_t rep_stride, void* stream) {
+    if (!values || !returns || !out || rows_per_chunk <= 0 || n_chunks <= 0 || n_mb <= 0 || n_rep <= 0) return B200RL_EINVAL;
+    cudaStream_t s = as_stream(stream);
+    if (mask)
+        explained_variance_kernel<true><<<n_mb, 1024, 0, s>>>(values, returns, mask, rows_per_chunk, n_chunks, chunk_stride, mb_offset, out,
+                                                             out_stride, n_rep, rep_stride);
+    else
+        explained_variance_kernel<false><<<n_mb, 1024, 0, s>>>(values, returns, mask, rows_per_chunk, n_chunks, chunk_stride, mb_offset, out,
+                                                              out_stride, n_rep, rep_stride);
+    B200RL_LAUNCH_CHECK();
+    return B200RL_OK;
+}
 
 B200RL_EXPORT int b200rl_prepare_batch_f32(const float* values, const float* returns, const float* mask,
                                            const double* partials, int n_partials,

@@ -12,6 +12,7 @@ from ._lib import lib, check, ptr, B200RLError
 ACT = {'None': 0, None: 0, 'none': 0, 'elu': 1, 'relu': 2, 'tanh': 3}
 # streaming multiprocessors of the H100 SXM: sizes the host buffers that hold one row per CTA of a grid capped at one CTA per SM
 NUM_SMS = 132
+STAT_SUMMASK, STAT_CLIPFRAC, STAT_EXPVAR = 5, 6, 9      # stats-row columns (include/b200rl.h B200RL_STAT_*)
 
 
 class LossCfg(ctypes.Structure):
@@ -113,6 +114,14 @@ def prepare_batch(values, returns, mask, partials, n_partials, vms_mean, vms_var
 def adv_ema_normalize(advs, partials, n_partials, ema_state, ema_step, decay, training=True):
     check(lib.b200rl_adv_ema_normalize_f32(ptr(advs), advs.numel(), ptr(partials), n_partials, ptr(ema_state), ptr(ema_step),
                                            float(decay), int(training), _stream()), 'adv_ema_normalize')
+
+
+def explained_variance(values, returns, mask, H, N, envs_per_mb, out, n_rep=1):
+    """explained variance of every whole-env minibatch of the [H, N] arena into out[i] (out: 1-D view, any stride); with n_rep > 1
+    the value is repeated at out[k * n_mb + i] (one stats row per mini-epoch)"""
+    n_mb, s = N // envs_per_mb, out.stride(0)
+    check(lib.b200rl_explained_variance_f32(ptr(values), ptr(returns), ptr(mask), envs_per_mb, H, N, n_mb, envs_per_mb, ptr(out), s,
+                                            n_rep, n_mb * s, _stream()), 'explained_variance')
 
 
 def batch_moments(values, returns, mask, partials):
