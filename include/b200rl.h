@@ -190,6 +190,23 @@ int b200rl_lstm_cell_fwd_f32(float* gates, const float* cin, float* c_out, float
 int b200rl_lstm_cell_bwd_f32(const float* gates_act, const float* c_t, const float* cin, const float* dH, int scatter_rpc,
                              int64_t scatter_stride, const float* dhin_next, const float* dcin_next, const uint8_t* done_next,
                              int done_rpc, int64_t done_stride, float* dgates, float* dcin, int S, int Hd, void* stream);
+/* LSTM cell + LayerNorm of its output (rnn.layer_norm: True; torch LayerNorm(Hd), eps 1e-5, biased variance; fp32):
+ *  cell_ln_fwd: cell_fwd's maths and arguments (h_out = raw h, the carries are raw as well) plus y = LN(h) * ln_w + ln_b into
+ *               y_out [S,Hd] (dense) and / or y_scatter (MLP-order rows as cell_fwd's h_scatter; at least one of the two), and the
+ *               row statistics mean [S], rstd [S] (optional, both or neither) for the backward.
+ *  cell_ln_bwd: dy = dY[scatter row] (scatter_rpc = S, scatter_stride = 0 for dense rows); h is recomputed from gates_act / c_t;
+ *               dh = LN backward of dy + dhin_next*(1-done_next), then cell_bwd's maths -> dgates, dcin.  dgamma / dbeta of the
+ *               step as n_splits row-split partials at dgamma_part / dbeta_part + p*split_stride (no atomics; sum them with
+ *               b200rl_reduce_splits_f32). */
+int b200rl_lstm_cell_ln_fwd_f32(float* gates, const float* cin, float* c_out, float* h_out, float* y_out, float* y_scatter,
+                                int scatter_rpc, int64_t scatter_stride, float* hin_next, float* cin_next, const uint8_t* done_next,
+                                int done_rpc, int64_t done_stride, const float* ln_w, const float* ln_b, float* mean, float* rstd,
+                                int S, int Hd, void* stream);
+int b200rl_lstm_cell_ln_bwd_f32(const float* gates_act, const float* c_t, const float* cin, const float* dY, int scatter_rpc,
+                                int64_t scatter_stride, const float* dhin_next, const float* dcin_next, const uint8_t* done_next,
+                                int done_rpc, int64_t done_stride, const float* ln_w, const float* mean, const float* rstd,
+                                float* dgamma_part, float* dbeta_part, int64_t split_stride, int n_splits, float* dgates, float* dcin,
+                                int S, int Hd, void* stream);
 /* train-time reset flags of an RNN policy on a next_step-autoreset env (a2c_common.py:1180-1191):
  * out[t, n] = dones[t, n] | (t > 0 && valid[t - 1, n] == 0)   ([H, N] contiguous) */
 int b200rl_rnn_train_dones_u8(const uint8_t* dones, const float* valid, uint8_t* out, int H, int N, void* stream);

@@ -296,6 +296,9 @@ class A2CAgent(A2CBase):
             self.t_gates, self.t_hin, self.t_cin, self.t_c = f(T, S, 4 * Hd), f(T, S, Hd), f(T, S, Hd), f(T, S, Hd)
             self.t_hdense, self.t_hmlp, self.t_dHmlp = f(S, Hd), f(mb, Hd), f(mb, Hd)
             self.t_dgates, self.t_dhin, self.t_dcin = f(S, 4 * Hd), f(S, Hd), f(2, S, Hd)
+            if m.rnn_layer_norm:     # LayerNorm(h): the rollout's normalised output, the window's per-step row statistics for BPTT
+                self.r_y = f(N, Hd)
+                self.t_mean, self.t_rstd = f(T, S), f(T, S)
         self.gae_partials = torch.zeros((N + 63) // 64, 8, dtype=torch.float64, device=dev)
         self.loss_partials = torch.zeros(max((mb + 127) // 128, ops.NUM_SMS), ops.loss_partial_stride(), dtype=torch.float64, device=dev)
         self.n_updates = self.mini_epochs_num * self.num_minibatches
@@ -551,11 +554,15 @@ class A2CAgent(A2CBase):
         return (m.running_mean_std.mean_f32, m.running_mean_std.std_f32) if self.normalize_input else (None, None)
 
     def _lstm_step(self, obs, h_in, c_in, h_out, c_out):
-        """one LSTM step for all N envs (seq_length 1, models.py -> network_builder.py:452-492 -> recurrent.py): returns h_out"""
+        """one LSTM step for all N envs (seq_length 1, models.py -> network_builder.py:452-492 -> recurrent.py): returns h_out, or its
+        LayerNorm (in self.r_y) with rnn.layer_norm"""
         m, N = self.model, self.num_actors
         nm, ns = self._norm() if m.rnn_before_mlp else (None, None)      # after the MLP the LSTM reads the trunk output
         self._lin_fwd(obs, m.W_ih, m.b_ih, self.r_gates, 0, x_ld=m.rnn_in, norm_mean=nm, norm_std=ns, M=N)
         self._lin_fwd(h_in, m.W_hh, m.b_hh, self.r_gates, 0, M=N, accumulate=True)
+        if m.rnn_layer_norm:     # the trunk / heads read LayerNorm(h); h_out / c_out stay the raw carried states
+            ops.lstm_cell_ln_fwd(self.r_gates, c_in, c_out, h_out, m.ln_w, m.ln_b, N, m.rnn_units, y_out=self.r_y)
+            return self.r_y
         ops.lstm_cell_fwd(self.r_gates, c_in, c_out, h_out, N, m.rnn_units)
         return h_out
 
@@ -837,6 +844,13 @@ class A2CAgent(A2CBase):
                            norm_mean=nm, norm_std=ns, M=S)
             self._lin_fwd(self.t_hin[t], m.W_hh, m.b_hh, self.t_gates[t], 0, M=S, accumulate=True)
             last = t == T - 1
+            if m.rnn_layer_norm:     # the MLP-order rows get LayerNorm(h); the carries stay raw; mean / rstd kept for the backward
+                ops.lstm_cell_ln_fwd(self.t_gates[t], self.t_cin[t], self.t_c[t], self.t_hdense, m.ln_w, m.ln_b, S, Hd,
+                                     y_scatter=self.t_hmlp[t * epm:], scatter_rpc=epm, scatter_stride=T * epm,
+                                     hin_next=None if last else self.t_hin[t + 1], cin_next=None if last else self.t_cin[t + 1],
+                                     done_next=None if last else dn[t + 1, e0:], done_rpc=epm, done_stride=T * N,
+                                     mean=self.t_mean[t], rstd=self.t_rstd[t])
+                continue
             ops.lstm_cell_fwd(self.t_gates[t], self.t_cin[t], self.t_c[t], self.t_hdense, S, Hd,
                               h_scatter=self.t_hmlp[t * epm:], scatter_rpc=epm, scatter_stride=T * epm,
                               hin_next=None if last else self.t_hin[t + 1], cin_next=None if last else self.t_cin[t + 1],
@@ -853,11 +867,20 @@ class A2CAgent(A2CBase):
         dn = self.rnn_dones_buf if self.rnn_dones_buf is not None else self.dones_buf
         for t in range(T - 1, -1, -1):
             last = t == T - 1
-            ops.lstm_cell_bwd(self.t_gates[t], self.t_c[t], self.t_cin[t], self.t_dgates, self.t_dcin[t & 1], S, Hd,
-                              dH=self.t_dHmlp[t * epm:], scatter_rpc=epm, scatter_stride=T * epm,
-                              dhin_next=None if last else self.t_dhin, dcin_next=None if last else self.t_dcin[(t + 1) & 1],
-                              done_next=None if last else dn[t + 1, e0:], done_rpc=epm, done_stride=T * N)
             row = t * Ssp
+            if m.rnn_layer_norm:
+                # t_dHmlp holds dL/dy; dgamma / dbeta of step t go to the same split rows as this step's W_ih / W_hh partials
+                o_lnw, o_lnb = m.layout['ln_w'][0], m.layout['ln_b'][0]
+                ops.lstm_cell_ln_bwd(self.t_gates[t], self.t_c[t], self.t_cin[t], self.t_dHmlp[t * epm:], m.ln_w, self.t_mean[t],
+                                     self.t_rstd[t], self.part[row, o_lnw:], self.part[row, o_lnb:], Ssp, self.t_dgates,
+                                     self.t_dcin[t & 1], S, Hd, scatter_rpc=epm, scatter_stride=T * epm,
+                                     dhin_next=None if last else self.t_dhin, dcin_next=None if last else self.t_dcin[(t + 1) & 1],
+                                     done_next=None if last else dn[t + 1, e0:], done_rpc=epm, done_stride=T * N, split_stride=P)
+            else:
+                ops.lstm_cell_bwd(self.t_gates[t], self.t_c[t], self.t_cin[t], self.t_dgates, self.t_dcin[t & 1], S, Hd,
+                                  dH=self.t_dHmlp[t * epm:], scatter_rpc=epm, scatter_stride=T * epm,
+                                  dhin_next=None if last else self.t_dhin, dcin_next=None if last else self.t_dcin[(t + 1) & 1],
+                                  done_next=None if last else dn[t + 1, e0:], done_rpc=epm, done_stride=T * N)
             xin, xstride = (self.obses[t, e0:], T * N) if m.rnn_before_mlp else (self.ta[-1][t * epm:], T * epm)
             self._lin_bww(self.t_dgates, xin, self.part[row, o_wih:], self.part[row, o_bih:], m.rnn_in, 4 * Hd, Ssp,
                                   rows_per_chunk=epm, chunk_stride=xstride, x_ld=m.rnn_in, norm_mean=nm, norm_std=ns, M=S, split_stride=P)

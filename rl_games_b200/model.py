@@ -10,6 +10,7 @@ arenas, so the optimiser, the gradient all-reduce and the checkpoint code each t
 
     [ sigma(A) | W_1 | b_1 | ... | W_L | b_L | W_head(A+1, H_L) | b_head(A+1) ]   (row 0 of the head = value)
 
+An LSTM adds ``W_ih | W_hh | b_ih | b_hh`` after ``sigma``, and with ``rnn.layer_norm`` its LayerNorm's ``ln_w | ln_b`` after those.
 A state-dependent sigma head (``fixed_sigma: False``) is A more head rows, ``W_head(1+2A, H_L) | b_head(1+2A)`` = (value, mu, sigma);
 the leading ``sigma(A)`` block then stays in the arena as dead space that is always exactly zero (no state-dict key, no Adam state,
 no gradient), so every offset convention of the fixed-sigma layout holds for both.
@@ -248,6 +249,7 @@ class FlatParamModel:
 class B200Model(FlatParamModel):
     RNN_KEYS = ('a2c_network.rnn.rnn.weight_ih_l0', 'a2c_network.rnn.rnn.weight_hh_l0', 'a2c_network.rnn.rnn.bias_ih_l0',
                 'a2c_network.rnn.rnn.bias_hh_l0')
+    LN_KEYS = ('a2c_network.layer_norm.weight', 'a2c_network.layer_norm.bias')
 
     def __init__(self, network_params, obs_dim, act_dim, device, normalize_input, normalize_value, value_size=1,
                  seed=None):
@@ -280,10 +282,12 @@ class B200Model(FlatParamModel):
         self.rnn_units = 0
         if 'rnn' in network_params:
             rnn = network_params['rnn']
-            if rnn.get('name') != 'lstm' or rnn.get('layers', 1) != 1 or rnn.get('layer_norm', False) \
+            if rnn.get('name') != 'lstm' or rnn.get('layers', 1) != 1 \
                     or rnn.get('concat_input', False) or rnn.get('concat_output', False):
-                raise NotImplementedError("rnn: only a single-layer 'lstm' (no layer_norm / concat) is on the B200 hot path")
+                raise NotImplementedError("rnn: only a single-layer 'lstm' (optionally layer-normed; no concat) is on the B200 hot path")
             self.rnn_units = int(rnn['units'])
+        # rnn.layer_norm (network_builder.py:279-280, :485-486): LayerNorm(rnn_units) of the LSTM output rows; the carried (h, c) stay raw
+        self.rnn_layer_norm = bool(self.rnn_units and network_params['rnn'].get('layer_norm', False))
         # placement (network_builder.py:253-272): before_mlp True = obs -> LSTM -> MLP -> heads (BASELINE configs[3]); False (the reference
         # default) = obs -> MLP -> LSTM -> heads.  Same parameter names and order either way, different shapes.
         self.rnn_before_mlp = bool(network_params.get('rnn', {}).get('before_mlp', False)) if self.rnn_units else True
@@ -321,6 +325,8 @@ class B200Model(FlatParamModel):
         self.rnn_in = (self.D if self.rnn_before_mlp else self.units[-1]) if Hd else 0      # input width of the LSTM
         if Hd:
             sizes += [('W_ih', (4 * Hd, self.rnn_in)), ('W_hh', (4 * Hd, Hd)), ('b_ih', (4 * Hd,)), ('b_hh', (4 * Hd,))]
+            if self.rnn_layer_norm:
+                sizes += [('ln_w', (Hd,)), ('ln_b', (Hd,))]
         ins = Hd if (Hd and self.rnn_before_mlp) else self.D
         for i, u in enumerate(self.units):
             sizes += [(f'W{i}', (u, ins)), (f'b{i}', (u,))]
@@ -345,6 +351,8 @@ class B200Model(FlatParamModel):
             self.sigma_chain = torch.ones(self.A, dtype=torch.float32, device=self.device)
         if self.rnn_units:
             self.W_ih, self.W_hh, self.b_ih, self.b_hh = (self.view(n) for n in ('W_ih', 'W_hh', 'b_ih', 'b_hh'))
+        self.ln_w = self.view('ln_w') if self.rnn_layer_norm else None
+        self.ln_b = self.view('ln_b') if self.rnn_layer_norm else None
         self.mlp_in = self.rnn_units if (self.rnn_units and self.rnn_before_mlp) else self.D
         self.W_head, self.b_head = self.view('W_head'), self.view('b_head')
         self.grad_mask = None
@@ -417,6 +425,8 @@ class B200Model(FlatParamModel):
             k = 1.0 / math.sqrt(Hd)
             for n, shp in (('W_ih', (4 * Hd, self.rnn_in)), ('W_hh', (4 * Hd, Hd)), ('b_ih', (4 * Hd,)), ('b_hh', (4 * Hd,))):
                 cpu[n] = torch.empty(*shp).uniform_(-k, k)
+            if self.rnn_layer_norm:      # torch.nn.LayerNorm's own init; the mlp initializer does not touch it
+                cpu['ln_w'], cpu['ln_b'] = torch.ones(Hd), torch.zeros(Hd)
         mu_init = space.get('mu_init', {'name': 'default'})
         if self.separate:       # every Linear of both trunks and both heads is initialised on its own (true fan-in), written into its block
             blocks = self._param_views(self.flat)[1:]               # actor W, b ... critic W, b ... value W, b, mu W, b
@@ -484,7 +494,7 @@ class B200Model(FlatParamModel):
         return self
 
     def parameters(self):
-        """Reference parameter order (optimizer state is index-keyed): sigma, actor_mlp.*, value.*, mu.* (state-dependent head:
+        """Reference parameter order (optimizer state is index-keyed): sigma, actor_mlp.*, [rnn.rnn.*, layer_norm.*], value.*, mu.* (state-dependent head:
         actor_mlp.*, value.*, mu.*, sigma.weight, sigma.bias)"""
         return self._param_views(self.flat)
 
@@ -496,6 +506,8 @@ class B200Model(FlatParamModel):
             out += [self.view(f'W{i}', arena), self.view(f'b{i}', arena)]
         if self.rnn_units:   # registration order in A2CBuilder.Network.__init__: actor_mlp placeholder precedes self.rnn
             out += [self.view(n, arena) for n in ('W_ih', 'W_hh', 'b_ih', 'b_hh')]
+            if self.rnn_layer_norm:      # self.layer_norm is registered right after self.rnn
+                out += [self.view('ln_w', arena), self.view('ln_b', arena)]
         wh, bh = self.view('W_head', arena), self.view('b_head', arena)
         A = self.A
         out += [wh[:1], bh[:1], wh[1:A + 1], bh[1:A + 1]]
@@ -519,7 +531,7 @@ class B200Model(FlatParamModel):
         return out
 
     def param_names(self):
-        """state-dict keys of _param_views, in the same order: sigma, actor_mlp.*, [critic_mlp.*], [rnn.*], value.*, mu.*; a
+        """state-dict keys of _param_views, in the same order: sigma, actor_mlp.*, [critic_mlp.*], [rnn.*], [layer_norm.*], value.*, mu.*; a
         state-dependent head: actor_mlp.*, value.*, mu.*, sigma.weight, sigma.bias"""
         if not self.fixed_sigma:
             keys = [f'a2c_network.actor_mlp.{2 * i}.{t}' for i in range(len(self.trunk_units)) for t in ('weight', 'bias')]
@@ -531,6 +543,8 @@ class B200Model(FlatParamModel):
                 keys += [f'a2c_network.{trunk}.{2 * i}.weight', f'a2c_network.{trunk}.{2 * i}.bias']
         if self.rnn_units:
             keys += list(self.RNN_KEYS)
+        if self.rnn_layer_norm:
+            keys += list(self.LN_KEYS)
         return keys + ['a2c_network.value.weight', 'a2c_network.value.bias', 'a2c_network.mu.weight', 'a2c_network.mu.bias']
 
     def load_state_dict(self, sd, strict=True):

@@ -545,6 +545,25 @@ def lstm_cell_bwd(gates_act, c_t, cin, dgates, dcin, S, Hd, dH=None, scatter_rpc
           'lstm_cell_bwd')
 
 
+def lstm_cell_ln_fwd(gates, cin, c_out, h_out, ln_w, ln_b, S, Hd, y_out=None, y_scatter=None, scatter_rpc=0, scatter_stride=0, hin_next=None,
+                     cin_next=None, done_next=None, done_rpc=0, done_stride=0, mean=None, rstd=None):
+    """lstm_cell_fwd plus y = LayerNorm(h) (rnn.layer_norm) into y_out (dense) and / or y_scatter; h_out and the carries stay raw"""
+    check(lib.b200rl_lstm_cell_ln_fwd_f32(ptr(gates), ptr(cin), ptr(c_out), ptr(h_out), ptr(y_out), ptr(y_scatter), scatter_rpc,
+                                          scatter_stride, ptr(hin_next), ptr(cin_next), ptr(done_next), done_rpc, done_stride, ptr(ln_w),
+                                          ptr(ln_b), ptr(mean), ptr(rstd), S, Hd, _stream()),
+          'lstm_cell_ln_fwd')
+
+
+def lstm_cell_ln_bwd(gates_act, c_t, cin, dY, ln_w, mean, rstd, dgamma_part, dbeta_part, n_splits, dgates, dcin, S, Hd, scatter_rpc=0,
+                     scatter_stride=0, dhin_next=None, dcin_next=None, done_next=None, done_rpc=0, done_stride=0, split_stride=0):
+    """backward of lstm_cell_ln_fwd: dY = dL/dy (scatter rows; dense when scatter_rpc is 0); dgamma / dbeta as n_splits row-split partials"""
+    check(lib.b200rl_lstm_cell_ln_bwd_f32(ptr(gates_act), ptr(c_t), ptr(cin), ptr(dY), scatter_rpc if scatter_rpc > 0 else S,
+                                          scatter_stride if scatter_rpc > 0 else 0, ptr(dhin_next), ptr(dcin_next), ptr(done_next), done_rpc,
+                                          done_stride, ptr(ln_w), ptr(mean), ptr(rstd), ptr(dgamma_part), ptr(dbeta_part), split_stride,
+                                          n_splits, ptr(dgates), ptr(dcin), S, Hd, _stream()),
+          'lstm_cell_ln_bwd')
+
+
 def rnn_train_dones(dones_u8, valid, out_u8):
     H, N = dones_u8.shape
     check(lib.b200rl_rnn_train_dones_u8(ptr(dones_u8), ptr(valid), ptr(out_u8), H, N, _stream()), 'rnn_train_dones')

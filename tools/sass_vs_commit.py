@@ -21,7 +21,8 @@ def funcs(obj):
             cur = re.sub(r'_GLOBAL__N__[0-9a-f]+_\d+_\w+?_cu_[0-9a-f]+', 'NS', m.group(1))
             out[cur] = []
         elif cur is not None:
-            ln = re.sub(r'/\*[0-9a-f]{4,}\*/', '', line).strip()
+            # addresses dropped, whitespace collapsed: a longer object widens cuobjdump's address column, which pads every line
+            ln = re.sub(r'\s+', ' ', re.sub(r'/\*[0-9a-f]{4,}\*/', '', line)).strip()
             if ln:
                 out[cur].append(ln)
     return out
