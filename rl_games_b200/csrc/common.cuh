@@ -79,6 +79,12 @@ __device__ __forceinline__ void block_sum_d(double (&v)[NV], double* sm) {
 }
 
 // ---- Philox4x32-10 (Salmon et al.), counter-based so launches are CUDA-graph replayable ----------
+// Counter layout: ctr_lo = row (env index), ctr_hi = bit fields that must never overlap, or two draws would share a stream.
+//   policy samplers (rollout.cu, mlp_tc.cu, discrete.cu): epoch << 20 | step << 4 | q,  step < 2^16, q < 16:
+//     Gaussian heads q = 0..7 (four normals per q, up to 32 actions), categorical heads q = 8 + j (j < CAT_MAXH = 8)
+//   synthetic env (rollout.cu synth_env_step_kernel, its own keys): epoch << 20 | step << 10 | q, step < 2^10,
+//     q < 2^9 (feature group of four), bit 9 set for the done draw
+// tests/_philox_ref.py restates this generator and the mappings below bit for bit on the host.
 struct Philox4 { uint32_t x, y, z, w; };
 __device__ __forceinline__ Philox4 philox4x32_10(uint64_t ctr_lo, uint64_t ctr_hi, uint64_t key) {
     uint32_t c0 = (uint32_t)ctr_lo, c1 = (uint32_t)(ctr_lo >> 32), c2 = (uint32_t)ctr_hi, c3 = (uint32_t)(ctr_hi >> 32);

@@ -687,6 +687,11 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
                         p.la.old_sigma[ar * p.A + j] = sSig[j];
                         const int c = 1 + j;
                         *reinterpret_cast<__nv_bfloat16*>(gd + tile_off(row, c >> 3, 2048u, 128u) + (c & 7) * 2) = __float2bfloat16_rn(dmu);
+                    } else if (j < 15) {
+                        // columns A+1..15 meet the zero rows of the packed W_head in the backward's first MMA: they must be 0, not
+                        // whatever the buffer held before (0 x NaN = NaN)
+                        const int c = 1 + j;
+                        *reinterpret_cast<__nv_bfloat16*>(gd + tile_off(row, c >> 3, 2048u, 128u) + (c & 7) * 2) = __float2bfloat16_rn(0.f);
                     }
                 }
                 if (h == 0) {
