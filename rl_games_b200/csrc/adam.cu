@@ -6,6 +6,7 @@
 // and the result is deterministic; the last CTA to finish advances (step, lr).
 #include "common.cuh"
 #include "loss_math.cuh"
+#include "tc_common.cuh"
 #include <cuda_bf16.h>
 #include <string.h>
 
@@ -372,6 +373,7 @@ __global__ void __launch_bounds__(1024) reduce_adam_kernel(const float* __restri
     }
     RA_STAMP(1);      // loss finalisation done (CTA 0 does none in the single-GPU edition: it is the last CTA's job)
     // ---- 1b. my slice of the flat gradient: sum over the splits, KG k-groups per element ----
+    const uint64_t pol = tc::l2_policy_first();       // the split rows are read once, here
     if (vec4) {
         // 16-byte edition (split rows and slice bounds are 4-float aligned): 4x the bytes in flight per thread -- the pass is
         // latency-bound (~232 KB of L2-resident partials per CTA).  Entries < A or >= n inside a group are loaded but ignored.
@@ -385,17 +387,17 @@ __global__ void __launch_bounds__(1024) reduce_adam_kernel(const float* __restri
                 const float* src = part + i;
                 int k = kg;
                 for (; k + 3 * KG < n_splits; k += 4 * KG) {
-                    const float4 v0 = __ldcg(reinterpret_cast<const float4*>(src + (int64_t)k * split_stride));
-                    const float4 v1 = __ldcg(reinterpret_cast<const float4*>(src + (int64_t)(k + KG) * split_stride));
-                    const float4 v2 = __ldcg(reinterpret_cast<const float4*>(src + (int64_t)(k + 2 * KG) * split_stride));
-                    const float4 v3 = __ldcg(reinterpret_cast<const float4*>(src + (int64_t)(k + 3 * KG) * split_stride));
+                    const float4 v0 = tc::ldcg_hint(reinterpret_cast<const float4*>(src + (int64_t)k * split_stride), pol);
+                    const float4 v1 = tc::ldcg_hint(reinterpret_cast<const float4*>(src + (int64_t)(k + KG) * split_stride), pol);
+                    const float4 v2 = tc::ldcg_hint(reinterpret_cast<const float4*>(src + (int64_t)(k + 2 * KG) * split_stride), pol);
+                    const float4 v3 = tc::ldcg_hint(reinterpret_cast<const float4*>(src + (int64_t)(k + 3 * KG) * split_stride), pol);
                     s0.x += v0.x; s0.y += v0.y; s0.z += v0.z; s0.w += v0.w;
                     s1.x += v1.x; s1.y += v1.y; s1.z += v1.z; s1.w += v1.w;
                     s2.x += v2.x; s2.y += v2.y; s2.z += v2.z; s2.w += v2.w;
                     s3.x += v3.x; s3.y += v3.y; s3.z += v3.z; s3.w += v3.w;
                 }
                 for (; k < n_splits; k += KG) {
-                    const float4 v0 = __ldcg(reinterpret_cast<const float4*>(src + (int64_t)k * split_stride));
+                    const float4 v0 = tc::ldcg_hint(reinterpret_cast<const float4*>(src + (int64_t)k * split_stride), pol);
                     s0.x += v0.x; s0.y += v0.y; s0.z += v0.z; s0.w += v0.w;
                 }
             }
@@ -428,12 +430,12 @@ __global__ void __launch_bounds__(1024) reduce_adam_kernel(const float* __restri
                 const float* src = part + i;
                 int k = kg;
                 for (; k + 3 * KG < n_splits; k += 4 * KG) {
-                    s0 += __ldcg(src + (int64_t)k * split_stride);
-                    s1 += __ldcg(src + (int64_t)(k + KG) * split_stride);
-                    s2 += __ldcg(src + (int64_t)(k + 2 * KG) * split_stride);
-                    s3 += __ldcg(src + (int64_t)(k + 3 * KG) * split_stride);
+                    s0 += tc::ldcg_hint(src + (int64_t)k * split_stride, pol);
+                    s1 += tc::ldcg_hint(src + (int64_t)(k + KG) * split_stride, pol);
+                    s2 += tc::ldcg_hint(src + (int64_t)(k + 2 * KG) * split_stride, pol);
+                    s3 += tc::ldcg_hint(src + (int64_t)(k + 3 * KG) * split_stride, pol);
                 }
-                for (; k < n_splits; k += KG) s0 += __ldcg(src + (int64_t)k * split_stride);
+                for (; k < n_splits; k += KG) s0 += tc::ldcg_hint(src + (int64_t)k * split_stride, pol);
             }
             sred[tid] = (s0 + s1) + (s2 + s3);
             __syncthreads();
@@ -444,6 +446,19 @@ __global__ void __launch_bounds__(1024) reduce_adam_kernel(const float* __restri
                 a0 = fmaf(g * gs, g * gs, a0);
             }
             __syncthreads();
+        }
+    }
+    // ---- 1b'. this CTA was the only reader of its slice of every split row, and every load of it has returned (the sums are in
+    //      shared memory, behind the pass's barrier): drop those lines from L2 instead of writing them back.  Only the 128-byte lines
+    //      that lie wholly inside the slice, so that a neighbouring CTA's slice never loses a line it has yet to read.  The next
+    //      writer is the backward kernel's flush.  Multi-GPU: `part` is this rank's own; the exchange buffers are left alone.
+    if (i1 > i0) {
+        const int warp = tid >> 5;
+        for (int k = warp; k < n_splits; k += 32) {
+            const uintptr_t a = reinterpret_cast<uintptr_t>(part + (int64_t)k * split_stride + i0),
+                            b = reinterpret_cast<uintptr_t>(part + (int64_t)k * split_stride + i1);
+            const uintptr_t lo = (a + 127) & ~(uintptr_t)127, hi = b & ~(uintptr_t)127;
+            if (hi > lo) tc::l2_discard(reinterpret_cast<void*>(lo), hi - lo);
         }
     }
     if (MULTI) {

@@ -52,6 +52,17 @@ __device__ __forceinline__ void bulk_g2s(void* sdst, const void* gsrc, uint32_t 
 __device__ __forceinline__ void bulk_s2g(void* gdst, const void* ssrc, uint32_t bytes) {
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(ssrc)), "r"(bytes) : "memory");
 }
+// the same copies with an L2 cache policy (tc_common.cuh: l2_policy_first / l2_policy_last)
+__device__ __forceinline__ void bulk_g2s(void* sdst, const void* gsrc, uint32_t bytes, uint64_t* bar, uint64_t pol) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(smem_u32(sdst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_s2g(void* gdst, const void* ssrc, uint32_t bytes, uint64_t pol) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(gdst), "r"(smem_u32(ssrc)), "r"(bytes),
+                 "l"(pol)
+                 : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 
@@ -445,7 +456,9 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
             const int m0 = blockIdx.x * 128;
             const uint32_t bytes = (uint32_t)min(128, p.M - m0) * p.D * 4u;
             mbar_expect_tx(&bars[5], bytes);
-            bulk_g2s(sXraw, p.obs + chunk_row(m0, p.rows_per_chunk, p.chunk_stride) * p.D, bytes, &bars[5]);
+            const float* src = p.obs + chunk_row(m0, p.rows_per_chunk, p.chunk_stride) * p.D;
+            if constexpr (TRAIN) bulk_g2s(sXraw, src, bytes, &bars[5], l2_policy_first());    // next read: the next mini-epoch
+            else bulk_g2s(sXraw, src, bytes, &bars[5]);
         }
     }
     TSTAMP();   // barriers initialised, first X tile requested
@@ -460,13 +473,21 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
         } else {
         // one barrier per consumer so that layer 1 starts as soon as W1 (32 KB of the 114 KB) has landed
         mbar_expect_tx(&bars[0], N::W1_BYTES);
-        bulk_g2s(sW1, p.wpack + N::W1_OFF, N::W1_BYTES, &bars[0]);
+        if constexpr (TRAIN) bulk_g2s(sW1, p.wpack + N::W1_OFF, N::W1_BYTES, &bars[0], l2_policy_last());
+        else bulk_g2s(sW1, p.wpack + N::W1_OFF, N::W1_BYTES, &bars[0]);
         }
         mbar_expect_tx(&bars[6], N::W2_BYTES);
-        bulk_g2s(sW2, p.wpack + N::W2_OFF, N::W2_BYTES, &bars[6]);
         mbar_expect_tx(&bars[7], N::W3_BYTES + N::WH_BYTES);
-        bulk_g2s(sW3, p.wpack + N::W3_OFF, N::W3_BYTES, &bars[7]);
-        bulk_g2s(sWh, p.wpack + N::WH_OFF, N::WH_BYTES, &bars[7]);
+        if constexpr (TRAIN) {      // every CTA of this kernel and of the backward reads the packed weights
+            const uint64_t pol = l2_policy_last();
+            bulk_g2s(sW2, p.wpack + N::W2_OFF, N::W2_BYTES, &bars[6], pol);
+            bulk_g2s(sW3, p.wpack + N::W3_OFF, N::W3_BYTES, &bars[7], pol);
+            bulk_g2s(sWh, p.wpack + N::WH_OFF, N::WH_BYTES, &bars[7], pol);
+        } else {
+            bulk_g2s(sW2, p.wpack + N::W2_OFF, N::W2_BYTES, &bars[6]);
+            bulk_g2s(sW3, p.wpack + N::W3_OFF, N::W3_BYTES, &bars[7]);
+            bulk_g2s(sWh, p.wpack + N::WH_OFF, N::WH_BYTES, &bars[7]);
+        }
     }
     // every global load of the prologue lands in a register first -- ONE memory round trip -- then the shared-memory stores
     {
@@ -528,14 +549,15 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
         TSTAMP();   // X staged
         if (TRAIN && p.xt) {      // keep the normalised bf16 tile for the weight-gradient kernel (16 B per thread-iteration, coalesced)
             uint4* gx = reinterpret_cast<uint4*>(p.xt + (size_t)tile * N::X_BYTES);
-            for (int i = tid; i < (int)N::X_BYTES / 16; i += FWD_THREADS) gx[i] = reinterpret_cast<const uint4*>(sXA2)[i];
+            const uint64_t pol = l2_policy_last();      // read back by the backward of this minibatch
+            for (int i = tid; i < (int)N::X_BYTES / 16; i += FWD_THREADS) st_hint_u128(gx + i, reinterpret_cast<const uint4*>(sXA2)[i], pol);
         }
         // ---------------- layer 1: a1[128, U1] = act(X . W1^T + b1) ----------------
         layer1_frag<N>(uXA2, smem_u32(sW1), sB1, sA1, nullptr);
         fence_async_smem();
         __syncthreads();
         if (TRAIN && tid == 0) {      // the global a1 tile is byte for byte the shared one
-            bulk_s2g(p.act1 + (size_t)tile * N::A1_BYTES, sA1, N::A1_BYTES);
+            bulk_s2g(p.act1 + (size_t)tile * N::A1_BYTES, sA1, N::A1_BYTES, l2_policy_last());
             bulk_commit();
         }
         }   // !XL1
@@ -555,7 +577,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
         fence_async_smem();
         __syncthreads();
         if (tid == 0 && TRAIN) {
-            bulk_s2g(p.act2 + (size_t)tile * N::A2_BYTES, sXA2, N::A2_BYTES);
+            bulk_s2g(p.act2 + (size_t)tile * N::A2_BYTES, sXA2, N::A2_BYTES, l2_policy_last());
             bulk_commit();
         }
         if (XL1 && tid == 0 && tile + (int)gridDim.x < n_tiles) {
@@ -568,7 +590,9 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
             const int m1 = (tile + gridDim.x) * 128;
             const uint32_t bytes = (uint32_t)min(128, p.M - m1) * p.D * 4u;
             mbar_expect_tx(&bars[5], bytes);
-            bulk_g2s(sXraw, p.obs + chunk_row(m1, p.rows_per_chunk, p.chunk_stride) * p.D, bytes, &bars[5]);
+            const float* src = p.obs + chunk_row(m1, p.rows_per_chunk, p.chunk_stride) * p.D;
+            if constexpr (TRAIN) bulk_g2s(sXraw, src, bytes, &bars[5], l2_policy_first());
+            else bulk_g2s(sXraw, src, bytes, &bars[5]);
         }
         TSTAMP();   // layer 2 done
         // ---------------- layer 3: a3[128, U3] = act(a2 . W3^T + b3), warpgroup (mh, nh): [64 x 32] ----------------
@@ -586,7 +610,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
         fence_async_smem();
         __syncthreads();
         if (TRAIN && tid == 0) {
-            bulk_s2g(p.act3 + (size_t)tile * N::A3_BYTES, sA3, N::A3_BYTES);
+            bulk_s2g(p.act3 + (size_t)tile * N::A3_BYTES, sA3, N::A3_BYTES, l2_policy_last());
             bulk_commit();
         }
         TSTAMP();   // layer 3 done
@@ -648,6 +672,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
             __syncthreads();
             TSTAMP();   // loss phase A done
             uint8_t* gd = p.dhead + (size_t)tile * N::DH_BYTES;
+            const uint64_t pol_dh = l2_policy_last();      // d_head: read back by the backward
             if (live) {
                 float sz2 = 0.f, kl = 0.f, bl = 0.f;
 #pragma unroll
@@ -686,12 +711,12 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
                         p.la.old_mu[ar * p.A + j] = mu;               // new mu/sigma overwrite the old ones (datasets.py:33-43)
                         p.la.old_sigma[ar * p.A + j] = sSig[j];
                         const int c = 1 + j;
-                        *reinterpret_cast<__nv_bfloat16*>(gd + tile_off(row, c >> 3, 2048u, 128u) + (c & 7) * 2) = __float2bfloat16_rn(dmu);
+                        st_hint_u16(gd + tile_off(row, c >> 3, 2048u, 128u) + (c & 7) * 2, __bfloat16_as_ushort(__float2bfloat16_rn(dmu)), pol_dh);
                     } else if (j < 15) {
                         // columns A+1..15 meet the zero rows of the packed W_head in the backward's first MMA: they must be 0, not
                         // whatever the buffer held before (0 x NaN = NaN)
                         const int c = 1 + j;
-                        *reinterpret_cast<__nv_bfloat16*>(gd + tile_off(row, c >> 3, 2048u, 128u) + (c & 7) * 2) = __float2bfloat16_rn(0.f);
+                        st_hint_u16(gd + tile_off(row, c >> 3, 2048u, 128u) + (c & 7) * 2, 0, pol_dh);
                     }
                 }
                 if (h == 0) {
@@ -706,7 +731,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
                         const float g1 = 2.0f * e1, g2 = (delta >= -p.cfg.e_clip && delta <= p.cfg.e_clip) ? 2.0f * e2 : 0.0f;
                         dc = (l1 > l2) ? g1 : ((l1 < l2) ? g2 : 0.5f * (g1 + g2));
                     } else { const float e1 = ret - val; c_loss = e1 * e1; dc = -2.0f * e1; }
-                    *reinterpret_cast<__nv_bfloat16*>(gd + tile_off(row, 0, 2048u, 128u)) = __float2bfloat16_rn(w * 0.5f * p.cfg.critic_coef * dc);
+                    st_hint_u16(gd + tile_off(row, 0, 2048u, 128u), __bfloat16_as_ushort(__float2bfloat16_rn(w * 0.5f * p.cfg.critic_coef * dc)), pol_dh);
                     const float lr_ = old_nlp - nlp;
                     const float clipped = (lr_ < p.cfg.log_lo || lr_ > p.cfg.log_hi) ? 1.f : 0.f;
                     sc[0] += w * a_loss; sc[1] += w * c_loss; sc[2] += w * sSig[4 * p.A + 1]; sc[3] += w * bl; sc[4] += w * kl;
@@ -714,7 +739,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_tc_kernel(const FwdArg
                 }
             } else if (h < 2) {
                 // padded rows of a partial tile: zero d_head so the backward kernels see no contribution
-                *reinterpret_cast<uint4*>(gd + tile_off(row, h, 2048u, 128u)) = make_uint4(0, 0, 0, 0);
+                st_hint_u128(gd + tile_off(row, h, 2048u, 128u), make_uint4(0, 0, 0, 0), pol_dh);
             }
         } else if (h == 0) {
             float head[16];
@@ -862,16 +887,17 @@ __device__ __forceinline__ void load_act_frag(uint32_t (&ua)[NS / 4], const uint
     }
 }
 // delta = dpre * act'(a) on the fragment, rounded to bf16 pairs and stored at the fragment's own positions of the shared delta tile
-// (operand of the next MMAs) and / or the global one
+// (operand of the next MMAs) and / or the global one (stored with evict_last: phase 2 of the same CTA reads it back)
 template <int NS>
 __device__ __forceinline__ void delta_epilogue(const float (&d)[NS / 2], const uint32_t (&ua)[NS / 4], uint8_t* sT, uint8_t* gT, uint32_t off0) {
+    const uint64_t pol = gT ? l2_policy_last() : 0;
 #pragma unroll
     for (int i = 0; i < NS / 4; ++i) {
         const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&ua[i]));
         const __nv_bfloat162 o = __floats2bfloat162_rn(mul_act_grad(d[2 * i], a.x), mul_act_grad(d[2 * i + 1], a.y));
         const uint32_t off = off0 + (i >> 1) * 2048u + (i & 1) * 128u;
         if (sT) *reinterpret_cast<uint32_t*>(sT + off) = *reinterpret_cast<const uint32_t*>(&o);
-        if (gT) *reinterpret_cast<uint32_t*>(gT + off) = *reinterpret_cast<const uint32_t*>(&o);
+        if (gT) st_hint_u32(gT + off, *reinterpret_cast<const uint32_t*>(&o), pol);
     }
 }
 // one tile's column sums added to the running bias-gradient sums in shared memory (each sum has one owning thread).  colsum8 keeps its
@@ -887,19 +913,21 @@ __device__ __forceinline__ void bias_colsum(const uint8_t* sT, int tid, float* s
         for (int j = 0; j < 8; ++j) sSum[g * 8 + j] += s[j];
     }
 }
+// The flushes store the split-gradient rows with evict_last: the optimiser's reducer, the next kernel, reads them back.
 __device__ __forceinline__ void flush_bias(const float* sSum, int n, float* dst, int tid) {
-    if (tid < n) dst[tid] = sSum[tid];
+    if (tid < n) st_hint_u32(dst + tid, __float_as_uint(sSum[tid]), l2_policy_last());
 }
 // a [64 x NS] fragment of a transposed weight gradient into the split-gradient row: element (in index i, out index o) ->
 // dst[o * ld + i] for i < ni, o < no; i0 / o0 = indices of d[0].  A warp writes 4 runs of 8 consecutive floats per store.
 template <int NS>
 __device__ __forceinline__ void flush_frag(const float (&d)[NS / 2], float* dst, int ld, int i0, int o0, int ni, int no) {
+    const uint64_t pol = l2_policy_last();
 #pragma unroll
     for (int j = 0; j < NS / 8; ++j) {
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
             const int i = i0 + (e >> 1) * 8, o = o0 + 8 * j + (e & 1);
-            if (i < ni && o < no) dst[o * ld + i] = d[4 * j + e];
+            if (i < ni && o < no) st_hint_u32(dst + o * ld + i, __float_as_uint(d[4 * j + e]), pol);
         }
     }
 }
@@ -929,16 +957,17 @@ __device__ __forceinline__ void bwd1_body(const Bwd1Args& p, uint8_t* smem) {
     __syncthreads();
     pdl_sync();      // everything above is CTA-local; all global traffic comes after the predecessor (the forward kernel) completed
     if (tid == 0) {
+        const uint64_t pol_w = l2_policy_last(), pol_t = l2_policy_first();     // d_head / a3 / a2: this is their last read
         mbar_expect_tx(&bars[0], N::WH_BYTES + N::W3_BYTES + N::W2_BYTES);
-        bulk_g2s(sWh, p.wpack + N::WH_OFF, N::WH_BYTES, &bars[0]);
-        bulk_g2s(sW3, p.wpack + N::W3_OFF, N::W3_BYTES, &bars[0]);
-        bulk_g2s(sW2, p.wpack + N::W2_OFF, N::W2_BYTES, &bars[0]);
+        bulk_g2s(sWh, p.wpack + N::WH_OFF, N::WH_BYTES, &bars[0], pol_w);
+        bulk_g2s(sW3, p.wpack + N::W3_OFF, N::W3_BYTES, &bars[0], pol_w);
+        bulk_g2s(sW2, p.wpack + N::W2_OFF, N::W2_BYTES, &bars[0], pol_w);
         if ((int)blockIdx.x < n_tiles) {      // first tile's operands
             const int tile = blockIdx.x;
             mbar_expect_tx(&bars[1], N::DH_BYTES + N::A3_BYTES + N::A2_BYTES);
-            bulk_g2s(sDH, p.dhead + (size_t)tile * N::DH_BYTES, N::DH_BYTES, &bars[1]);
-            bulk_g2s(sA3, p.act3 + (size_t)tile * N::A3_BYTES, N::A3_BYTES, &bars[1]);
-            bulk_g2s(sA2, p.act2 + (size_t)tile * N::A2_BYTES, N::A2_BYTES, &bars[1]);
+            bulk_g2s(sDH, p.dhead + (size_t)tile * N::DH_BYTES, N::DH_BYTES, &bars[1], pol_t);
+            bulk_g2s(sA3, p.act3 + (size_t)tile * N::A3_BYTES, N::A3_BYTES, &bars[1], pol_t);
+            bulk_g2s(sA2, p.act2 + (size_t)tile * N::A2_BYTES, N::A2_BYTES, &bars[1], pol_t);
         }
     }
     // operand views (tc_common.cuh): K-major rows advance by ARS per 8, MN-major columns by the column-group stride per 8
@@ -998,10 +1027,11 @@ __device__ __forceinline__ void bwd1_body(const Bwd1Args& p, uint8_t* smem) {
             // d_head / a3 / a2 tiles are dead (MMAs a, b completed, epilogue reads fenced + synced): prefetch the next tile's
             // operands so that they land while d1pre and its epilogue run
             const int nt = tile + gridDim.x;
+            const uint64_t pol_t = l2_policy_first();
             mbar_expect_tx(&bars[1], N::DH_BYTES + N::A3_BYTES + N::A2_BYTES);
-            bulk_g2s(sDH, p.dhead + (size_t)nt * N::DH_BYTES, N::DH_BYTES, &bars[1]);
-            bulk_g2s(sA3, p.act3 + (size_t)nt * N::A3_BYTES, N::A3_BYTES, &bars[1]);
-            bulk_g2s(sA2, p.act2 + (size_t)nt * N::A2_BYTES, N::A2_BYTES, &bars[1]);
+            bulk_g2s(sDH, p.dhead + (size_t)nt * N::DH_BYTES, N::DH_BYTES, &bars[1], pol_t);
+            bulk_g2s(sA3, p.act3 + (size_t)nt * N::A3_BYTES, N::A3_BYTES, &bars[1], pol_t);
+            bulk_g2s(sA2, p.act2 + (size_t)nt * N::A2_BYTES, N::A2_BYTES, &bars[1], pol_t);
         }
         {   // ---- d1pre = d2 . W2 in two column halves: the epilogue of the first runs while the chain of the second is in flight ----
             const uint8_t* ga1 = p.act1 + (size_t)tile * N::A1_BYTES;      // a1 is read from its global tile
@@ -1101,11 +1131,13 @@ __device__ __forceinline__ void bwd2_body(const Bwd2Args& p, uint8_t* smem) {
         __syncthreads();      // the previous tile's MMAs (every warpgroup waited for its own) and bias sums have read the operand tiles
         TSTAMP();   // tile start
         if (tid == 0) {
+            // the last reads of these tiles in the update -- except d1 of the wide geometry, which l1_wgrad_tc_kernel reads next
+            const uint64_t pol = l2_policy_first(), pol_d1 = XL1 ? l2_policy_last() : pol;
             mbar_expect_tx(&bars[0], N::A2_BYTES + 2 * N::A1_BYTES + (x_from_fwd ? N::X_BYTES : 0u));
-            bulk_g2s(sD2, p.delta2 + (size_t)tile * N::A2_BYTES, N::A2_BYTES, &bars[0]);
-            bulk_g2s(sD1, p.delta1 + (size_t)tile * N::A1_BYTES, N::A1_BYTES, &bars[0]);
-            bulk_g2s(sA1, p.act1 + (size_t)tile * N::A1_BYTES, N::A1_BYTES, &bars[0]);
-            if (x_from_fwd) bulk_g2s(sX, p.xt + (size_t)tile * N::X_BYTES, N::X_BYTES, &bars[0]);
+            bulk_g2s(sD2, p.delta2 + (size_t)tile * N::A2_BYTES, N::A2_BYTES, &bars[0], pol);
+            bulk_g2s(sD1, p.delta1 + (size_t)tile * N::A1_BYTES, N::A1_BYTES, &bars[0], pol_d1);
+            bulk_g2s(sA1, p.act1 + (size_t)tile * N::A1_BYTES, N::A1_BYTES, &bars[0], pol);
+            if (x_from_fwd) bulk_g2s(sX, p.xt + (size_t)tile * N::X_BYTES, N::X_BYTES, &bars[0], pol);
         }
         if constexpr (!XL1) {
             if (!x_from_fwd) {

@@ -52,6 +52,64 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         "DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 
+// ---- L2 cache policies ---------------------------------------------------------------------------------
+// A minibatch update moves ~200 MB through the 50 MB L2.  Scratch that a later kernel of the same update reads back (activation and
+// delta tiles, split-gradient rows) is stored with evict_last; data read for the last time in the update (observation rows, the
+// tiles' last reads, the split-gradient rows in the reducer) is loaded with evict_first, so that it does not push out the former.
+// The hints change where lines live, never what a load returns.
+__device__ __forceinline__ uint64_t l2_policy_first() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_last() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint32_t ld_hint_u32(const void* p, uint64_t pol) {
+    uint32_t v;
+    asm volatile("ld.global.nc.L2::cache_hint.b32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ void st_hint_u32(void* p, uint32_t v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.b32 [%0], %1, %2;" ::"l"(p), "r"(v), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_hint_u16(void* p, uint16_t v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.b16 [%0], %1, %2;" ::"l"(p), "h"(v), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_hint_u128(void* p, uint4 v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "l"(pol)
+                 : "memory");
+}
+// cached-at-L2-only loads (__ldcg) with a policy
+__device__ __forceinline__ float ldcg_hint(const float* p, uint64_t pol) {
+    float v;
+    asm volatile("ld.global.cg.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ float4 ldcg_hint(const float4* p, uint64_t pol) {
+    float4 v;
+    asm volatile("ld.global.cg.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol));
+    return v;
+}
+
+// Lines of [p, p + bytes), both ends 128-byte aligned, whose data no one will read again: dropped from L2 without a write-back to
+// HBM.  Run by the 32 lanes of one warp.  A read of a discarded byte before its next write returns an indeterminate value, so the
+// caller must be the last reader.  The B200RL_L2_DISCARD_POISON build (a test library, never the product) stores 0xFF bytes there
+// instead -- NaN in fp32 and bf16 -- so that a read after the discard fails deterministically instead of by timing.
+__device__ __forceinline__ void l2_discard(void* p, size_t bytes) {
+    for (size_t o = (size_t)(threadIdx.x & 31) * 128u; o < bytes; o += 32u * 128u) {
+#ifdef B200RL_L2_DISCARD_POISON
+        uint4* q = reinterpret_cast<uint4*>(static_cast<uint8_t*>(p) + o);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) q[i] = make_uint4(~0u, ~0u, ~0u, ~0u);
+#else
+        asm volatile("discard.global.L2 [%0], 128;" ::"l"(static_cast<uint8_t*>(p) + o) : "memory");
+#endif
+    }
+}
+
 // ---- wgmma: D[64 x n] += A[64 x 16] . B[16 x n], bf16 operands from shared memory, fp32 accumulators in the registers of one
 //      warpgroup (thread t: rows 16 (t/32) + (t%32)/4 and +8, columns 8j + 2 (t%4) + {0, 1} -> d[4j .. 4j+3]).
 //      TA / TB = 1 select the MN-major view of the operand.
