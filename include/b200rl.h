@@ -340,6 +340,16 @@ int b200rl_categorical_loss_f32(const float* logits, int ld, int K, int n_heads,
                                 const float* inv_count_dev, float* d_logits, int d_ld, float* d_value, int dv_ld,
                                 double* partials, int max_partials, int* n_blocks_out_host, void* stream);
 
+/* Central value with a multi-agent env (agents > 1; central_value.py:224-244).
+ *  b200rl_cv_value_broadcast_f32: out[e*agents + a] = denorm(val[e]) for the N envs' critic values val[N] (de-normalised with the value
+ *    normaliser's vms_mean / vms_var when normalize_value), i.e. every agent row of an env gets its env's value.
+ *  b200rl_cv_gather_agent0_f32: the critic's [H, N] old values / returns from the actor's [H, N*agents] arena in the reference's
+ *    update_multiagent_tensors order: dst[t*N + e] = src[t*N*agents + e*agents] (agent 0 of every env). */
+int b200rl_cv_value_broadcast_f32(const float* val, const double* vms_mean, const double* vms_var, int normalize_value,
+                                  float* out, int N, int agents, void* stream);
+int b200rl_cv_gather_agent0_f32(const float* src_a, const float* src_b, float* dst_a, float* dst_b, int H, int N, int agents,
+                                void* stream);
+
 /* Value-only loss head of the central value network (central_value.py:276-301).  NOT YET RUN ON HARDWARE (see csrc/critic.cu).
  * loss = (masked) mean of critic_loss(old_values_n, values, e_clip, returns_n, clip_value); d_value[m*dv_ld] = its gradient;
  * arena tensors addressed as chunk_row(m, rows_per_chunk, chunk_stride); partial rows of 8 doubles {w*loss, mask, w, 0...}. */
@@ -489,6 +499,22 @@ int b200rl_post_step_f32(const float* rewards, const void* dones, int dones_is_u
                          float* ep_state, double* meter, int games_to_track,
                          double* scratch, int scratch_blocks, int* counter, int N,
                          const b200rl_shaper_cfg* cfg_host, void* stream);
+
+/* Multi-agent post-step (env_info['agents'] = agents > 1; N = envs * agents rows, a2c_common.py:1039-1051): the same shaping and
+ * per-row episode accumulators as b200rl_post_step_f32, but only every agents-th done row in index order (the reference's
+ * dones.nonzero()[::agents]) updates the meters, and those rows' indices are written to sel_idx[0 .. *sel_count) (int64, ascending;
+ * sel_idx holds up to ceil(N / agents) entries).  current_* are zeroed on every done row.  Deterministic: a row's rank among the
+ * step's done rows is a device-wide ordered prefix count, and the meter partials are summed in tile order.
+ *  scratch: double[scratch_tiles*4], tile_status: uint64[scratch_tiles], scratch_tiles >= ceil(N / B200RL_POST_STEP_MA_TILE);
+ *  tile_status and counters int32[2] are zeroed once by the caller and re-armed by every launch. */
+#define B200RL_POST_STEP_MA_TILE 1024
+int b200rl_post_step_ma_f32(const float* rewards, const void* dones, int dones_is_u8, const void* time_outs,
+                            int time_outs_kind, const float* values_t, const float* valid_t,
+                            float* rewards_out_t, uint8_t* dones_cur, float* prev_dones_f32,
+                            float* ep_state, double* meter, int games_to_track,
+                            double* scratch, uint64_t* tile_status, int scratch_tiles, int* counters,
+                            int64_t* sel_idx, int* sel_count, int N, int agents,
+                            const b200rl_shaper_cfg* cfg_host, void* stream);
 
 /* Synthetic on-GPU measurement env (SURVEY.md 8d; not part of the reference): obs ~ N(0,1) (Philox),
  * reward = -||a||^2, done = (t >= max_len) | Bernoulli(p_done), time_out = (t>=max_len) & !terminated. */

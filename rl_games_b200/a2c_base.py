@@ -12,6 +12,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from . import ops
 from .common import (AdaptiveScheduler, IdentityScheduler, LinearScheduler, DefaultAlgoObserver, DefaultRewardsShaper,
                      create_vec_env, make_summary_writer)
 from .diagnostics import PpoDiagnostics, make_diagnostics, replay as replay_diagnostics
@@ -212,6 +213,26 @@ class A2CBase(CompileTolerantModel):
             self.mean_rewards = self.last_mean_rewards = -float('inf')
         self.algo_observer.after_clear_stats()
 
+    # =============================================================================== post env-step bookkeeping
+    def _post_step(self, rewards, dones, tout, t, N):
+        """shaped rewards into arena step t, episode accumulators and meters (a2c_common.py:1019-1051); with agents > 1 the meters see
+        every agents-th done row (dones.nonzero()[::agents])"""
+        valid_t = None if self.valid is None else self.valid[t]
+        if self.post_ma is None:
+            ops.post_step(rewards, dones, tout, self.values[t], valid_t, self.rewards[t], self.dones, self.prev_dones, self.ep_state,
+                          self.meter, self.games_to_track, self.post_scratch, self.counters[0:1], N, self.shaper_cfg)
+        else:
+            ops.post_step_ma(rewards, dones, tout, self.values[t], valid_t, self.rewards[t], self.dones, self.prev_dones, self.ep_state,
+                             self.meter, self.games_to_track, self.post_ma, N, self.num_agents, self.shaper_cfg)
+
+    def _done_indices(self):
+        """the reference's env_done_indices ([K, 1] int64, a2c_common.py:1039-1040) for an observer that wants them, as a tensor of its
+        own like the one nonzero() makes (the device list is rewritten by the next step); one host read"""
+        if self.post_ma is None:
+            return self.dones.nonzero(as_tuple=False)
+        sel_idx, sel_count = self.post_ma[3], self.post_ma[4]
+        return sel_idx[:int(sel_count.item())].unsqueeze(1).clone()
+
     # =============================================================================== multi-GPU stats sync
     def _stats_modules(self):
         mods = []
@@ -274,12 +295,14 @@ class A2CBase(CompileTolerantModel):
             should_exit = False
             if self.global_rank == 0:
                 self.diagnostics.epoch(self, current_epoch=epoch_num)
+                # a2c_common.py:1394-1398: frames count agent rows, the inference and total rates are per env (times scaled by agents)
+                scaled_time, scaled_play_time = self.num_agents * sum_time, self.num_agents * play_time
                 if self.print_stats:
                     st = max(step_time, 1e-9)
-                    print(f'fps step: {curr_frames / st:.0f} fps step and policy inference: {curr_frames / play_time:.0f} '
-                          f'fps total: {curr_frames / sum_time:.0f} epoch: {epoch_num:.0f}/{self.max_epochs:.0f} frames: {frame:.0f}')
+                    print(f'fps step: {curr_frames / st:.0f} fps step and policy inference: {curr_frames / scaled_play_time:.0f} '
+                          f'fps total: {curr_frames / scaled_time:.0f} epoch: {epoch_num:.0f}/{self.max_epochs:.0f} frames: {frame:.0f}')
                 self.write_stats(total_time, epoch_num, step_time, play_time, update_time, a_losses, c_losses, entropies, kls,
-                                 last_lr, lr_mul, frame, sum_time, play_time, curr_frames)
+                                 last_lr, lr_mul, frame, scaled_time, scaled_play_time, curr_frames)
                 mean_rewards = None
                 if self.game_rewards.current_size > 0:
                     mh = self._meter_host()[:3].astype(self.episode_summary_dtype)

@@ -173,6 +173,8 @@ class A2CAgent(A2CBase):
 
     def _parse_config(self, config):
         self.value_size = self.env_info.get('value_size', 1)
+        if self.value_size != 1:
+            raise NotImplementedError('value_size > 1 is not on the B200 hot path yet')
         self.observation_space = self.env_info['observation_space']
         if config.get('use_action_masks', False):
             raise NotImplementedError('action masks are a discrete-PPO feature')
@@ -181,9 +183,10 @@ class A2CAgent(A2CBase):
             raise NotImplementedError('central_value_config is served by rl_games_b200.agent_cv.A2CAgentCV: build the agent through '
                                       'rl_games_b200.register(runner) / rl_games_b200.runner.continuous_agent, which pick it')
         self.central_value_net = None
+        # multi-agent envs (a2c_common.py:340, :393, :556): every agent row is an actor row, so the arena has envs * agents rows in the
+        # env's row order and minibatches are slices of agent rows
         self.num_agents = self.env_info.get('agents', 1)
-        if self.num_agents != 1:
-            raise NotImplementedError('multi-agent envs are not on the B200 hot path yet')
+        self.num_rows = self.num_actors * self.num_agents
         if self.mask_autoreset_rows and self.num_agents > 1:
             raise ValueError("PPO next_step autoreset masking does not support multi-agent envs; "
                              "wrap the env with a same_step autoreset adapter instead")
@@ -217,7 +220,7 @@ class A2CAgent(A2CBase):
         """a2c_common.py:634-660 + experience.py:330-398: one time-major arena, zero-initialised."""
         if self._tensors_ready:
             return
-        H, N, D, A = self.horizon_length, self.num_actors, self.obs_shape[0], self.actions_num
+        H, N, D, A = self.horizon_length, self.num_rows, self.obs_shape[0], self.actions_num
         dev = self.device_t
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)   # noqa: E731
         self.obses = f(H, N, D)
@@ -338,6 +341,8 @@ class A2CAgent(A2CBase):
             self._merge_structs = [ops.make_obs_merge(self.mbmom[i], self.mb_shift, D, mb, r.running_mean, r.running_var, r.count,
                                                       r.mean_f32, r.std_f32) for i in range(self.num_minibatches)]
         self.post_scratch = torch.zeros(((N + 255) // 256) * 4, dtype=torch.float64, device=dev)
+        # multi-agent post-step: tile partials and status words, ticket counters, the step's selected done rows and their count
+        self.post_ma = ops.post_step_ma_buffers(N, self.num_agents, dev) if self.num_agents > 1 else None
         self.counters = torch.zeros(4, dtype=torch.int32, device=dev)
         if self.normalize_rms_advantage and not hasattr(self, 'adv_ema_state'):
             self.adv_ema_state = torch.zeros(2, dtype=torch.float32, device=dev)     # GeneralizedMovingStats: mean, mean of squares
@@ -556,7 +561,7 @@ class A2CAgent(A2CBase):
     def _lstm_step(self, obs, h_in, c_in, h_out, c_out):
         """one LSTM step for all N envs (seq_length 1, models.py -> network_builder.py:452-492 -> recurrent.py): returns h_out, or its
         LayerNorm (in self.r_y) with rnn.layer_norm"""
-        m, N = self.model, self.num_actors
+        m, N = self.model, self.num_rows
         nm, ns = self._norm() if m.rnn_before_mlp else (None, None)      # after the MLP the LSTM reads the trunk output
         self._lin_fwd(obs, m.W_ih, m.b_ih, self.r_gates, 0, x_ld=m.rnn_in, norm_mean=nm, norm_std=ns, M=N)
         self._lin_fwd(h_in, m.W_hh, m.b_hh, self.r_gates, 0, M=N, accumulate=True)
@@ -567,7 +572,7 @@ class A2CAgent(A2CBase):
         return h_out
 
     def _policy_step(self, obs, t, noise=None):
-        m, N, A = self.model, self.num_actors, self.actions_num
+        m, N, A = self.model, self.num_rows, self.actions_num
         if self.use_tc and not self.rollout_fp32:
             nm, ns = self._norm()
             ops.tc_mlp_fwd_rollout(obs, m.D, nm, ns, self.wpack, m.b, m.b_head, m.sigma, m.units, N, A,
@@ -601,7 +606,7 @@ class A2CAgent(A2CBase):
     def get_values(self, obs):
         """a2c_common.py:603-626"""
         o = obs['obs'] if isinstance(obs, dict) else obs
-        m, N, A = self.model, self.num_actors, self.actions_num
+        m, N, A = self.model, self.num_rows, self.actions_num
         if self.use_tc and not self.rollout_fp32:
             nm, ns = self._norm()
             ops.tc_mlp_fwd_rollout(o, m.D, nm, ns, self.wpack, m.b, m.b_head, m.sigma, m.units, N, A,
@@ -635,7 +640,7 @@ class A2CAgent(A2CBase):
     # =============================================================================== rollout
     def _rollout(self, noise=None):
         """a2c_common.py:985-1069 without the eager launches: obs copy, trunk, head+sample+store, env, post-step."""
-        H, N = self.horizon_length, self.num_actors
+        H, N = self.horizon_length, self.num_rows
         step_time = 0.0
         wants_idx = getattr(self.algo_observer, 'wants_done_indices', True)
         wants_infos = getattr(self.algo_observer, 'wants_infos', False)
@@ -659,14 +664,12 @@ class A2CAgent(A2CBase):
             self.obs, rewards, dones, infos = self.env_step(self.env_actions)
             step_time += time.perf_counter() - t0
             tout = infos.get('time_outs') if (self.value_bootstrap and isinstance(infos, dict)) else None
-            ops.post_step(rewards, dones, tout, self.values[t], None if self.valid is None else self.valid[t], self.rewards[t],
-                          self.dones, self.prev_dones, self.ep_state, self.meter, self.games_to_track, self.post_scratch,
-                          self.counters[0:1], N, self.shaper_cfg)
-            if self.is_rnn:     # zero the states of finished episodes (a2c_common.py:1150-1153)
+            self._post_step(rewards, dones, tout, t, N)
+            if self.is_rnn:     # zero the states of finished episodes (a2c_common.py:1150-1153): every done agent row
                 ops.rnn_mask_rows(self.rnn_h, N, 0, self.rnn_h, N, self.model.rnn_units, done=self.dones, done_rpc=N)
                 ops.rnn_mask_rows(self.rnn_c, N, 0, self.rnn_c, N, self.model.rnn_units, done=self.dones, done_rpc=N)
             if wants_idx:
-                self.algo_observer.process_infos(infos, self.dones.nonzero(as_tuple=False))
+                self.algo_observer.process_infos(infos, self._done_indices())
             elif wants_infos:       # observers that read the infos but not the done indices: no host sync
                 self.algo_observer.process_infos(infos, None)
         self.get_values(self.obs)
@@ -695,14 +698,14 @@ class A2CAgent(A2CBase):
             ops.adv_ema_normalize(self.advs_n, self.gae_partials, n_partials, self.adv_ema_state, self.adv_ema_step,
                                   self.adv_rms_momentum, training=True)
         if self.mask_autoreset_rows:
-            ops.mask_inv_counts(self.valid, self.horizon_length, self.num_actors, self.envs_per_mb, self.inv_counts)
+            ops.mask_inv_counts(self.valid, self.horizon_length, self.num_rows, self.envs_per_mb, self.inv_counts)
         if self.diag_on:
             # diagnostics/exp_var of every minibatch from the prepared dataset, into column B200RL_STAT_EXPVAR of each of its updates' rows
-            ops.explained_variance(self.old_values_n, self.returns_n, self.valid, self.horizon_length, self.num_actors, self.envs_per_mb,
+            ops.explained_variance(self.old_values_n, self.returns_n, self.valid, self.horizon_length, self.num_rows, self.envs_per_mb,
                                    self.stats[:, ops.STAT_EXPVAR], n_rep=self.mini_epochs_num)
         if self.use_mb_moments:
             # obs are fixed for the whole update phase: batch sums of every minibatch in ONE pass over the arena
-            ops.obs_mb_moments(self.obses, m.D, self.horizon_length, self.num_actors, self.envs_per_mb,
+            ops.obs_mb_moments(self.obses, m.D, self.horizon_length, self.num_rows, self.envs_per_mb,
                                m.running_mean_std.running_mean, self.mbmom, self.mb_shift, self.mom_scratch, self.mb_counters)
 
     def play_steps(self, noise=None):
@@ -725,7 +728,7 @@ class A2CAgent(A2CBase):
     def prepare_dataset(self, batch_dict):
         """a2c_common.py:1586-1660.  Accepts the dict from play_steps (possibly edited by the caller: edited or
         foreign tensors are scattered back into the arena first)."""
-        H, N = self.horizon_length, self.num_actors
+        H, N = self.horizon_length, self.num_rows
         unfl = lambda t: t.reshape(N, H, *t.shape[1:]).transpose(0, 1)   # noqa: E731
         ids = getattr(self, '_batch_dict_ids', {})
         dirty = False
@@ -746,7 +749,7 @@ class A2CAgent(A2CBase):
     # =============================================================================== update
     def _minibatch_update(self, i, u):
         """calc_gradients + trancate_gradients_and_step for minibatch i; u = flat update index (stats row)."""
-        m, H, N, A = self.model, self.horizon_length, self.num_actors, self.actions_num
+        m, H, N, A = self.model, self.horizon_length, self.num_rows, self.actions_num
         epm, mb = self.envs_per_mb, self.minibatch_size
         e0 = i * epm
         x = self.obses[0, e0:]
@@ -829,7 +832,7 @@ class A2CAgent(A2CBase):
     def _lstm_window_fwd(self, e0):
         """Training forward of the LSTM over the seq_length window of every sequence of the minibatch (network_builder.py:452-492,
         recurrent.py:26-58): sequences (j, env) in order j*epm + (env - e0); step t uses arena rows (j*T + t, env)."""
-        m, H, N, T = self.model, self.horizon_length, self.num_actors, self.seq_length
+        m, H, N, T = self.model, self.horizon_length, self.num_rows, self.seq_length
         epm, Hd = self.envs_per_mb, m.rnn_units
         S = epm * H // T
         nm, ns = self._norm() if m.rnn_before_mlp else (None, None)
@@ -859,7 +862,7 @@ class A2CAgent(A2CBase):
     def _lstm_window_bwd(self, e0):
         """BPTT over the window: cell backward, weight gradients of W_ih / W_hh (+ both biases) per step into their own split rows,
         dgrad through W_hh to the previous step."""
-        m, H, N, T = self.model, self.horizon_length, self.num_actors, self.seq_length
+        m, H, N, T = self.model, self.horizon_length, self.num_rows, self.seq_length
         epm, Hd, P, Ssp = self.envs_per_mb, m.rnn_units, m.num_params, self.n_splits
         S = epm * H // T
         nm, ns = self._norm() if m.rnn_before_mlp else (None, None)
@@ -897,7 +900,7 @@ class A2CAgent(A2CBase):
 
     def _minibatch_update_tc(self, i, u, x, e0):
         """bf16 wgmma edition: fused fwd+loss kernel, two backward kernels, split reduce, Adam, repack."""
-        m, H, N, A = self.model, self.horizon_length, self.num_actors, self.actions_num
+        m, H, N, A = self.model, self.horizon_length, self.num_rows, self.actions_num
         epm, mb, P = self.envs_per_mb, self.minibatch_size, self.model.num_params
         nm, ns = self._norm()
         nb = ops.tc_mlp_fwd_train(x, epm, N, m.D, nm, ns, self.wpack, m.b, m.b_head, m.sigma, m.units, mb, A, self.actions[0, e0:],

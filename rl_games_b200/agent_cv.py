@@ -49,7 +49,8 @@ class CentralValueNet(FlatParamModel):
         raise NotImplementedError('the central value net is a flat parameter arena driven by kernels (get_value / train_net); '
                                   'it has no module-style forward')
 
-    def __init__(self, cv_config, state_dim, num_actors, horizon, normalize_value, max_epochs, device, multi_gpu=False, world_size=1):
+    def __init__(self, cv_config, state_dim, num_actors, horizon, normalize_value, max_epochs, device, multi_gpu=False, world_size=1,
+                 num_agents=1):
         net = cv_config['network']
         self.multi_gpu, self.world_size = bool(multi_gpu) and world_size > 1, int(world_size)
         self.writter = None             # the agent's summary writer (central_value.py:79; the reference's spelling)
@@ -61,6 +62,8 @@ class CentralValueNet(FlatParamModel):
             raise NotImplementedError('central value network: a plain MLP is supported')
         self.act_id = ops.ACT[self.activation]
         self.S, self.N, self.H = int(state_dim), int(num_actors), int(horizon)
+        # multi-agent env: one state row per env; the value goes to the env's agent rows, the dataset is agent 0's (central_value.py:224-244)
+        self.agents = int(num_agents)
         self.device = torch.device(device)
         self.normalize_input, self.normalize_value = bool(cv_config['normalize_input']), bool(normalize_value)
         self.lr = float(cv_config['learning_rate'])
@@ -104,6 +107,8 @@ class CentralValueNet(FlatParamModel):
         self.grad = f(off)
         self.loss_partials = torch.zeros((mb + 255) // 256, 8, dtype=torch.float64, device=dev)
         self.inv_counts = f(self.num_minibatches)
+        if self.agents > 1:
+            self.old_values_n, self.returns_n = f(self.H, self.N), f(self.H, self.N)
         self.mom_scratch = torch.zeros(ops.NUM_SMS * 4 * 2 * self.S, dtype=torch.float64, device=dev)
         self.counters = torch.zeros(4, dtype=torch.int32, device=dev)
         self.opt_state = torch.tensor([self.lr, 0.0, 0.0, 0.0], dtype=torch.float64, device=dev)
@@ -140,10 +145,15 @@ class CentralValueNet(FlatParamModel):
             ops.linear_fwd(acts[i - 1], self.view(f'W{i}'), self.view(f'b{i}'), acts[i], self.act_id, M=M)
 
     def get_value(self, states, out):
-        """central_value.py:207-229 (eval mode): out[N] = denorm(critic(states))"""
+        """central_value.py:207-229 (eval mode): out[N] = denorm(critic(states)); with agents > 1, out[N * agents] = each env's value on
+        each of its agent rows"""
         self._trunk(states, self.r_act, self.N)
         ops.linear_fwd(self.r_act[-1], self.view('W_v'), self.view('b_v'), self.r_val, 0, M=self.N)
-        if self.normalize_value:
+        if self.agents > 1:
+            vm = self.value_mean_std
+            ops.cv_value_broadcast(self.r_val, vm.running_mean if vm else None, vm.running_var if vm else None, self.normalize_value, out,
+                                   self.N, self.agents)
+        elif self.normalize_value:
             vm = self.value_mean_std
             ops.normalize(self.r_val, vm.running_mean, vm.running_var, denorm=True, out=out.view(self.N, 1))
         else:
@@ -151,7 +161,11 @@ class CentralValueNet(FlatParamModel):
 
     # ---------------------------------------------------------------------------------------------- training (central_value.py:246-274)
     def train_net(self, old_values_n, returns_n, valid):
+        """old_values_n / returns_n: the actor's prepared [H, N * agents] arena; with agents > 1 the critic trains on agent 0's rows"""
         H, N, mb, epm, P, S_ = self.H, self.N, self.minibatch_size, self.envs_per_mb, self.num_params, self.n_splits
+        if self.agents > 1:
+            ops.cv_gather_agent0(old_values_n, returns_n, self.old_values_n, self.returns_n, H, N, self.agents)
+            old_values_n, returns_n = self.old_values_n, self.returns_n
         if valid is not None:
             ops.mask_inv_counts(valid, H, N, epm, self.inv_counts)
         rows = []
@@ -224,7 +238,8 @@ class A2CAgentCV(A2CAgent):
             raise NotImplementedError('only flat state spaces')
         self.state_shape = space.shape
         self.central_value_net = CentralValueNet(cv_config, space.shape[0], self.num_actors, self.horizon_length, self.normalize_value,
-                                                 self.max_epochs, self.device_t, multi_gpu=self.multi_gpu, world_size=self.world_size)
+                                                 self.max_epochs, self.device_t, multi_gpu=self.multi_gpu, world_size=self.world_size,
+                                                 num_agents=self.num_agents)
         self.central_value_net.writter = self.writer
         self.value_mean_std = self.central_value_net.value_mean_std                        # a2c_continuous.py:72-73
         self._states = None

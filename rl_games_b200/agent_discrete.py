@@ -120,8 +120,8 @@ class DiscreteA2CAgent(A2CBase):
         return mode
 
     def _parse_config(self, config):
-        if self.env_info.get('agents', 1) != 1 or self.env_info.get('value_size', 1) != 1:
-            raise NotImplementedError('multi-agent envs / value_size > 1')
+        if self.env_info.get('value_size', 1) != 1:
+            raise NotImplementedError('value_size > 1')
         if config.get('central_value_config') is not None:
             raise NotImplementedError('central_value_config')
         # options of the reference agent that change what a run does and are not built for the discrete path: refuse, never ignore
@@ -131,7 +131,12 @@ class DiscreteA2CAgent(A2CBase):
             if bad:
                 raise NotImplementedError(f'{key} is not built for the discrete B200 agent')
         self.has_central_value, self.central_value_net = False, None
-        self.num_agents, self.value_size = 1, 1
+        # multi-agent envs (the smac shape, a2c_common.py:340, :393): envs * agents independent actor rows, each with its own action mask
+        self.num_agents, self.value_size = self.env_info.get('agents', 1), 1
+        self.num_rows = self.num_actors * self.num_agents
+        if self.mask_autoreset_rows and self.num_agents > 1:
+            raise ValueError("PPO next_step autoreset masking does not support multi-agent envs; "
+                             "wrap the env with a same_step autoreset adapter instead")
         self.observation_space = self.env_info['observation_space']
         if type(self.observation_space).__name__ == 'Dict' or len(self.observation_space.shape) != 1:
             raise NotImplementedError('only flat Box observations')
@@ -168,7 +173,7 @@ class DiscreteA2CAgent(A2CBase):
     def init_tensors(self):
         if self._tensors_ready:
             return
-        H, N, D, K, m, mb = self.horizon_length, self.num_actors, self.obs_shape[0], self.actions_num, self.model, self.minibatch_size
+        H, N, D, K, m, mb = self.horizon_length, self.num_rows, self.obs_shape[0], self.actions_num, self.model, self.minibatch_size
         dev = self.device_t
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)   # noqa: E731
         self.obses = f(H, N, D)
@@ -205,6 +210,7 @@ class DiscreteA2CAgent(A2CBase):
         self.inv_counts = f(self.num_minibatches) if self.mask_autoreset_rows else None
         self.mom_scratch = torch.zeros(ops.NUM_SMS * 4 * 2 * D, dtype=torch.float64, device=dev)
         self.post_scratch = torch.zeros(((N + 255) // 256) * 4, dtype=torch.float64, device=dev)
+        self.post_ma = ops.post_step_ma_buffers(N, self.num_agents, dev) if self.num_agents > 1 else None
         self.counters = torch.zeros(4, dtype=torch.int32, device=dev)
         self.opt_state = torch.tensor([self.last_lr, 0.0, 0.0, 0.0], dtype=torch.float64, device=dev)
         self.adam_stats = f(16)
@@ -278,7 +284,7 @@ class DiscreteA2CAgent(A2CBase):
     def play_steps(self, u=None):
         """a2c_common.py:985-1069 for a discrete space; u: optional [H + 1, N] uniform tape (tests) -- else Philox."""
         self.init_tensors()
-        H, N, K, m = self.horizon_length, self.num_actors, self.actions_num, self.model
+        H, N, K, m = self.horizon_length, self.num_rows, self.actions_num, self.model
         vm = m.value_mean_std
         step_time = 0.0
         for t in range(H):
@@ -303,11 +309,9 @@ class DiscreteA2CAgent(A2CBase):
             tout = infos.get('time_outs') if (self.value_bootstrap and isinstance(infos, dict)) else None
             if tout is not None:
                 tout = self._to_dev(tout)
-            ops.post_step(rewards, dones, tout, self.values[t], None if self.valid is None else self.valid[t], self.rewards[t],
-                          self.dones, self.prev_dones, self.ep_state, self.meter, self.games_to_track, self.post_scratch,
-                          self.counters[0:1], N, self.shaper_cfg)
+            self._post_step(rewards, dones, tout, t, N)
             if getattr(self.algo_observer, 'wants_done_indices', True):
-                self.algo_observer.process_infos(infos, self.dones.nonzero(as_tuple=False))
+                self.algo_observer.process_infos(infos, self._done_indices())
             elif getattr(self.algo_observer, 'wants_infos', False):
                 self.algo_observer.process_infos(infos, None)
         # get_values (a2c_common.py:603-626): the reference's forward samples here too; only the value is used
@@ -335,16 +339,16 @@ class DiscreteA2CAgent(A2CBase):
         ops.prepare_batch(self.values, self.returns, self.valid, self.gae_partials, nb, s.running_mean, s.running_var, s.count,
                           self.old_values_n, self.returns_n, self.advs_n, self.normalize_value, self.normalize_advantage)
         if self.mask_autoreset_rows:
-            ops.mask_inv_counts(self.valid, self.horizon_length, self.num_actors, self.envs_per_mb, self.inv_counts)
+            ops.mask_inv_counts(self.valid, self.horizon_length, self.num_rows, self.envs_per_mb, self.inv_counts)
         if self.diag_on:        # diagnostics/exp_var of every minibatch from the prepared dataset
-            ops.explained_variance(self.old_values_n, self.returns_n, self.valid, self.horizon_length, self.num_actors, self.envs_per_mb,
+            ops.explained_variance(self.old_values_n, self.returns_n, self.valid, self.horizon_length, self.num_rows, self.envs_per_mb,
                                    self.diag_exp_var)
 
     # =============================================================================== update
     def _minibatch_update(self, i):
         """calc_gradients (a2c_discrete.py:121-209) + trancate_gradients_and_step for minibatch i; returns a device row
         [a_loss, c_loss, entropy, kl] (masked means)."""
-        m, H, N, K = self.model, self.horizon_length, self.num_actors, self.actions_num
+        m, H, N, K = self.model, self.horizon_length, self.num_rows, self.actions_num
         epm, mb, P, S = self.envs_per_mb, self.minibatch_size, self.model.num_params, self.n_splits
         e0 = i * epm
         x = self.obses[0, e0:]

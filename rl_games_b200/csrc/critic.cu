@@ -56,6 +56,35 @@ __global__ void __launch_bounds__(256) value_loss_kernel(const ValueLossArgs a, 
     }
 }
 
+// Multi-agent envs (agents = G > 1), central_value.py:224-226: the critic's value of env e (one state row per env), de-normalised with
+// the value normaliser when it is on (running_mean_std.py:104-106, as normalize_kernel's denorm), written to the G agent rows e*G .. e*G+G-1
+// of the actor's values[t] / last_values.  One thread per agent row.
+__global__ void __launch_bounds__(256) cv_value_broadcast_kernel(const float* __restrict__ val, const double* __restrict__ vms_mean,
+                                                                 const double* __restrict__ vms_var, int normalize_value,
+                                                                 float* __restrict__ out, int N, int G) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= N * G) return;
+    float v = val[r / G];
+    if (normalize_value) {
+        const float m = (float)vms_mean[0], s = __fsqrt_rn(__fadd_rn((float)vms_var[0], 1e-5f));
+        v = __fadd_rn(__fmul_rn(s, fminf(fmaxf(v, -5.0f), 5.0f)), m);
+    }
+    out[r] = v;
+}
+
+// central_value.py:235-244 update_multiagent_tensors: the actor's [H, N*G] old values and returns viewed as (N, G, H), transposed to
+// (G, N, H) and cut to the first N*H rows = agent 0 of every env; here as the critic's [H, N] arena: dst[t][e] = src[t][e*G].  (The
+// reference cuts its dones without the transpose; a feed-forward critic never reads them.)
+__global__ void __launch_bounds__(256) cv_gather_agent0_kernel(const float* __restrict__ src_a, const float* __restrict__ src_b,
+                                                               float* __restrict__ dst_a, float* __restrict__ dst_b, int H, int N, int G) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (int64_t)H * N) return;
+    const int64_t t = i / N, e = i - t * N;
+    const int64_t s = t * N * G + e * G;
+    dst_a[i] = src_a[s];
+    dst_b[i] = src_b[s];
+}
+
 }  // namespace
 
 B200RL_EXPORT int b200rl_value_loss_f32(const float* values, int value_ld, const float* old_values_n, const float* returns_n,
@@ -70,6 +99,27 @@ B200RL_EXPORT int b200rl_value_loss_f32(const float* values, int value_ld, const
     const ValueLossArgs a{values, value_ld, old_values_n, returns_n, mask, rows_per_chunk, chunk_stride, M, e_clip, clip_value, inv_count_dev,
                           d_value, dv_ld};
     value_loss_kernel<<<blocks, 256, 0, as_stream(stream)>>>(a, partials);
+    B200RL_LAUNCH_CHECK();
+    return B200RL_OK;
+}
+
+B200RL_EXPORT int b200rl_cv_value_broadcast_f32(const float* val, const double* vms_mean, const double* vms_var, int normalize_value,
+                                                float* out, int N, int agents, void* stream) {
+    if (!val || !out || N <= 0 || agents <= 0) return B200RL_EINVAL;
+    if (normalize_value && (!vms_mean || !vms_var)) return B200RL_EINVAL;
+    const int64_t rows = (int64_t)N * agents;
+    if (rows > INT32_MAX) return B200RL_EINVAL;
+    cv_value_broadcast_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, as_stream(stream)>>>(val, vms_mean, vms_var, normalize_value, out, N,
+                                                                                           agents);
+    B200RL_LAUNCH_CHECK();
+    return B200RL_OK;
+}
+
+B200RL_EXPORT int b200rl_cv_gather_agent0_f32(const float* src_a, const float* src_b, float* dst_a, float* dst_b, int H, int N, int agents,
+                                              void* stream) {
+    if (!src_a || !src_b || !dst_a || !dst_b || H <= 0 || N <= 0 || agents <= 0) return B200RL_EINVAL;
+    const int64_t total = (int64_t)H * N;
+    cv_gather_agent0_kernel<<<(unsigned)((total + 255) / 256), 256, 0, as_stream(stream)>>>(src_a, src_b, dst_a, dst_b, H, N, agents);
     B200RL_LAUNCH_CHECK();
     return B200RL_OK;
 }

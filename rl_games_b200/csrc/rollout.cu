@@ -216,6 +216,141 @@ __global__ void __launch_bounds__(256) post_step_kernel(
     }
 }
 
+// Multi-agent edition of post_step (a2c_common.py:1039-1051 with num_agents = G > 1): the step's done rows are ranked in index
+// order and only ranks 0, G, 2G, ... (all_done_indices[::G]) feed the meters and the selected-index list; current_* are zeroed on
+// every done row.  One pass: a CTA takes tiles in ticket order, ranks its rows with warp ballots, and gets the count of done rows
+// before its tile by decoupled look-back over the earlier tiles' status words -- the ranks depend on row order only, never on
+// scheduling.  A CTA waits only on tiles whose tickets were drawn before its own, so every tile it waits on is already running.
+// tile_status: u64 per tile, 0 = not published, else (flag << 62) | count (flag 1 = tile's own count, 2 = count through the tile).
+// The last CTA reduces the per-tile meter partials in tile order, writes sel_count and re-arms tile_status and the counters.
+constexpr int MA_THREADS = 256, MA_SLABS = 4, MA_TILE = MA_THREADS * MA_SLABS;
+static_assert(MA_TILE == B200RL_POST_STEP_MA_TILE, "include/b200rl.h states the tile size");
+constexpr unsigned long long MA_AGG = 1ull << 62, MA_INCL = 2ull << 62, MA_VAL = (1ull << 62) - 1;
+
+template <typename DT>
+__global__ void __launch_bounds__(MA_THREADS) post_step_ma_kernel(
+    const float* __restrict__ rewards, const DT* __restrict__ dones, const void* __restrict__ time_outs, int time_outs_kind,
+    const float* __restrict__ values_t, const float* __restrict__ valid_t, float* __restrict__ rewards_out_t,
+    uint8_t* __restrict__ dones_cur, float* __restrict__ prev_dones, float* __restrict__ ep_state, double* meter,
+    int games_to_track, double* scratch, unsigned long long* tile_status, int* counters, int64_t* __restrict__ sel_idx,
+    int* sel_count, int N, int G, ShaperDev c) {
+    __shared__ double sm[32 * 4];
+    __shared__ int slab_count[MA_SLABS][MA_THREADS / 32];
+    __shared__ int s_tile, s_excl, is_last;
+    pdl_sync();
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) s_tile = atomicAdd(counters, 1);
+    __syncthreads();
+    const int tile = s_tile;
+    float cr[MA_SLABS], cs[MA_SLABS], cl[MA_SLABS];
+    bool done[MA_SLABS];
+    unsigned ball[MA_SLABS];
+#pragma unroll
+    for (int k = 0; k < MA_SLABS; ++k) {
+        const int e = tile * MA_TILE + k * MA_THREADS + tid;
+        done[k] = false;
+        if (e < N) {
+            const float r = rewards[e];
+            float sh = __fmul_rn(__fadd_rn(r, c.shift_value), c.scale_value);
+            sh = fminf(fmaxf(sh, c.min_val), c.max_val);
+            if (c.log_val) sh = logf(sh);
+            if (c.value_bootstrap && time_outs_kind) {
+                const float to = time_outs_kind == 1 ? (float)((const uint8_t*)time_outs)[e] : ((const float*)time_outs)[e];
+                sh = __fadd_rn(sh, __fmul_rn(__fmul_rn(c.gamma, values_t[e]), to));
+            }
+            rewards_out_t[e] = sh;
+            const float live = valid_t ? valid_t[e] : 1.0f;
+            cr[k] = ep_state[e] + r * live;
+            cs[k] = ep_state[N + e] + sh * live;
+            cl[k] = ep_state[2 * N + e] + live;
+            const float d = (float)dones[e];
+            done[k] = d != 0.f;
+            const float nd = 1.0f - d;
+            ep_state[e] = cr[k] * nd; ep_state[N + e] = cs[k] * nd; ep_state[2 * N + e] = cl[k] * nd;
+            dones_cur[e] = done[k] ? 1 : 0;
+            if (prev_dones) prev_dones[e] = d;
+        }
+        ball[k] = __ballot_sync(0xffffffffu, done[k]);
+        if (lane == 0) slab_count[k][warp] = __popc(ball[k]);
+    }
+    __syncthreads();
+    // exclusive prefix over (slab, warp) in row order, in place; warp 0 lane i holds entry i of the 32
+    if (warp == 0) {
+        const int v = slab_count[lane / (MA_THREADS / 32)][lane % (MA_THREADS / 32)];
+        int incl = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+        }
+        slab_count[lane / (MA_THREADS / 32)][lane % (MA_THREADS / 32)] = incl - v;
+        const unsigned long long agg = (unsigned long long)__shfl_sync(0xffffffffu, incl, 31);
+        if (lane == 0) {
+            volatile unsigned long long* st = tile_status;
+            unsigned long long excl = 0;
+            if (tile == 0) {
+                st[0] = MA_INCL | agg;
+            } else {
+                st[tile] = MA_AGG | agg;
+                for (int j = tile - 1; j >= 0; --j) {
+                    unsigned long long w;
+                    do { w = st[j]; } while (w == 0ull);
+                    excl += w & MA_VAL;
+                    if ((w & ~MA_VAL) == MA_INCL) break;
+                }
+                st[tile] = MA_INCL | (excl + agg);
+            }
+            s_excl = (int)excl;
+        }
+    }
+    __syncthreads();
+    const unsigned lt = (1u << lane) - 1u;
+    double acc[4] = {0, 0, 0, 0};
+#pragma unroll
+    for (int k = 0; k < MA_SLABS; ++k) {
+        if (!done[k]) continue;
+        const int rank = s_excl + slab_count[k][warp] + __popc(ball[k] & lt);
+        if (rank % G == 0) {
+            sel_idx[rank / G] = (int64_t)(tile * MA_TILE + k * MA_THREADS + tid);
+            acc[0] += 1.0; acc[1] += cr[k]; acc[2] += cs[k]; acc[3] += cl[k];
+        }
+    }
+    block_sum_d<4>(acc, sm);
+    if (tid == 0) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) scratch[(int64_t)tile * 4 + i] = acc[i];
+    }
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) is_last = (atomicAdd(counters + 1, 1) == (int)gridDim.x - 1);
+    __syncthreads();
+    if (!is_last) return;
+    __threadfence();
+    double t[4] = {0, 0, 0, 0};
+    for (int b = tid; b < (int)gridDim.x; b += blockDim.x) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) t[i] += __ldcg(scratch + (int64_t)b * 4 + i);
+        tile_status[b] = 0ull;
+    }
+    block_sum_d<4>(t, sm);
+    if (tid == 0) {
+        const double n = t[0];
+        if (n > 0.0) {      // AverageMeter.update over the selected rows (torch_ext.py:333-342)
+            const double size = fmin(n, (double)games_to_track);
+            const double old_size = fmin((double)games_to_track - size, meter[3]);
+            const double size_sum = old_size + size;
+            meter[0] = (meter[0] * old_size + (t[1] / n) * size) / size_sum;
+            meter[1] = (meter[1] * old_size + (t[2] / n) * size) / size_sum;
+            meter[2] = (meter[2] * old_size + (t[3] / n) * size) / size_sum;
+            meter[3] = size_sum;
+            meter[4] += n;
+        }
+        *sel_count = (int)n;
+        counters[0] = 0;
+        counters[1] = 0;
+    }
+}
+
 // one thread per (env, group of 4 features)
 __global__ void __launch_bounds__(256) synth_env_step_kernel(const float* __restrict__ actions, float* __restrict__ obs,
                                                             float* __restrict__ rewards, uint8_t* __restrict__ dones,
@@ -341,6 +476,38 @@ B200RL_EXPORT int b200rl_post_step_f32(const float* rewards, const void* dones, 
     else
         le = launch_k(post_step_kernel<float>, dim3(blocks), dim3(256), 0, s, rewards, (const float*)dones, time_outs, time_outs_kind, values_t,
                       valid_t, rewards_out_t, dones_cur, prev_dones_f32, ep_state, meter, games_to_track, scratch, counter, N, c);
+    if (le != cudaSuccess) return (int)le;
+    return B200RL_OK;
+}
+
+B200RL_EXPORT int b200rl_post_step_ma_f32(const float* rewards, const void* dones, int dones_is_u8, const void* time_outs,
+                                          int time_outs_kind, const float* values_t, const float* valid_t,
+                                          float* rewards_out_t, uint8_t* dones_cur, float* prev_dones_f32,
+                                          float* ep_state, double* meter, int games_to_track,
+                                          double* scratch, uint64_t* tile_status, int scratch_tiles, int* counters,
+                                          int64_t* sel_idx, int* sel_count, int N, int agents,
+                                          const b200rl_shaper_cfg* cfg_host, void* stream) {
+    if (!rewards || !dones || !rewards_out_t || !dones_cur || !ep_state || !meter || !scratch || !tile_status || !counters ||
+        !sel_idx || !sel_count || !cfg_host || N <= 0 || agents <= 0)
+        return B200RL_EINVAL;
+    if (time_outs_kind && (!time_outs || !values_t)) return B200RL_EINVAL;
+    const int tiles = (N + MA_TILE - 1) / MA_TILE;
+    if (tiles > scratch_tiles) return B200RL_EINVAL;
+    ShaperDev c;
+    c.scale_value = cfg_host->scale_value; c.shift_value = cfg_host->shift_value; c.min_val = cfg_host->min_val;
+    c.max_val = cfg_host->max_val; c.gamma = cfg_host->gamma; c.log_val = cfg_host->log_val;
+    c.value_bootstrap = cfg_host->value_bootstrap;
+    cudaStream_t s = as_stream(stream);
+    unsigned long long* st = reinterpret_cast<unsigned long long*>(tile_status);
+    cudaError_t le;
+    if (dones_is_u8)
+        le = launch_k(post_step_ma_kernel<uint8_t>, dim3(tiles), dim3(MA_THREADS), 0, s, rewards, (const uint8_t*)dones, time_outs,
+                      time_outs_kind, values_t, valid_t, rewards_out_t, dones_cur, prev_dones_f32, ep_state, meter, games_to_track,
+                      scratch, st, counters, sel_idx, sel_count, N, agents, c);
+    else
+        le = launch_k(post_step_ma_kernel<float>, dim3(tiles), dim3(MA_THREADS), 0, s, rewards, (const float*)dones, time_outs,
+                      time_outs_kind, values_t, valid_t, rewards_out_t, dones_cur, prev_dones_f32, ep_state, meter, games_to_track,
+                      scratch, st, counters, sel_idx, sel_count, N, agents, c);
     if (le != cudaSuccess) return (int)le;
     return B200RL_OK;
 }

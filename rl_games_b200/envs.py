@@ -24,8 +24,10 @@ class SyntheticGPUEnv(IVecEnv):
     cuda_graph_capturable = True
 
     def __init__(self, config_name, num_actors, obs_dim=60, act_dim=8, max_len=100, p_done=0.01, seed=5,
-                 device='cuda:0', autoreset_mode='same_step', **kwargs):
-        self.N, self.D, self.A = int(num_actors), int(obs_dim), int(act_dim)
+                 device='cuda:0', autoreset_mode='same_step', agents=1, **kwargs):
+        # agents > 1: a multi-agent env of num_actors envs whose rows are num_actors * agents independent agent rows
+        self.agents = int(agents)
+        self.N, self.D, self.A = int(num_actors) * self.agents, int(obs_dim), int(act_dim)
         self.max_len, self.p_done, self._seed = int(max_len), float(p_done), int(seed)
         self.device = torch.device(device)
         self.autoreset_mode = autoreset_mode
@@ -68,6 +70,8 @@ class SyntheticGPUEnv(IVecEnv):
         info = {'observation_space': Box(-np.inf, np.inf, (self.D,)), 'action_space': Box(-1.0, 1.0, (self.A,))}
         if self.autoreset_mode != 'same_step':
             info['autoreset_mode'] = self.autoreset_mode
+        if self.agents > 1:
+            info['agents'] = self.agents
         return info
 
 

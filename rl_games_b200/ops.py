@@ -376,6 +376,49 @@ def post_step(rewards, dones, time_outs, values_t, valid_t, rewards_out_t, dones
                                    ctypes.addressof(cfg), _stream()), 'post_step')
 
 
+def cv_value_broadcast(val, vms_mean, vms_var, normalize_value, out, N, agents):
+    """out[e*agents + a] = the (de-normalised) critic value of env e"""
+    check(lib.b200rl_cv_value_broadcast_f32(ptr(val), ptr(vms_mean), ptr(vms_var), int(bool(normalize_value)), ptr(out), N, agents,
+                                            _stream()), 'cv_value_broadcast')
+
+
+def cv_gather_agent0(src_a, src_b, dst_a, dst_b, H, N, agents):
+    """critic rows [H, N] <- agent 0 of every env in the actor's [H, N*agents] arena (update_multiagent_tensors order)"""
+    check(lib.b200rl_cv_gather_agent0_f32(ptr(src_a), ptr(src_b), ptr(dst_a), ptr(dst_b), H, N, agents, _stream()), 'cv_gather_agent0')
+
+
+POST_STEP_MA_TILE = 1024        # include/b200rl.h B200RL_POST_STEP_MA_TILE
+
+
+def post_step_ma_buffers(N, agents, device):
+    """(scratch, tile_status, counters, sel_idx, sel_count) for post_step_ma over N rows, zeroed once"""
+    tiles = (N + POST_STEP_MA_TILE - 1) // POST_STEP_MA_TILE
+    z = lambda n, dt: torch.zeros(n, dtype=dt, device=device)     # noqa: E731
+    return (z(tiles * 4, torch.float64), z(tiles, torch.int64), z(2, torch.int32), z((N + agents - 1) // agents, torch.int64),
+            z(1, torch.int32))
+
+
+def post_step_ma(rewards, dones, time_outs, values_t, valid_t, rewards_out_t, dones_cur, prev_dones, ep_state, meter, games_to_track,
+                 bufs, N, agents, cfg):
+    """post_step over N = envs * agents rows; the meters see dones.nonzero()[::agents], whose indices land in bufs[3][:bufs[4]]"""
+    d_u8 = 1 if dones.dtype in (torch.uint8, torch.bool) else 0
+    if not d_u8 and dones.dtype != torch.float32:
+        dones = dones.float()
+    kind = 0
+    if time_outs is not None:
+        if time_outs.dtype in (torch.uint8, torch.bool):
+            kind = 1
+        else:
+            kind = 2
+            if time_outs.dtype != torch.float32:
+                time_outs = time_outs.float()
+    scratch, status, counters, sel_idx, sel_count = bufs
+    check(lib.b200rl_post_step_ma_f32(ptr(rewards), ptr(dones), d_u8, ptr(time_outs), kind, ptr(values_t), ptr(valid_t),
+                                      ptr(rewards_out_t), ptr(dones_cur), ptr(prev_dones), ptr(ep_state), ptr(meter),
+                                      games_to_track, ptr(scratch), ptr(status), status.numel(), ptr(counters), ptr(sel_idx),
+                                      ptr(sel_count), N, agents, ctypes.addressof(cfg), _stream()), 'post_step_ma')
+
+
 def synth_env_step(actions, obs, rewards, dones, time_outs, ep_t, N, D, A, max_len, p_done, seed, rng_epoch, step_index):
     check(lib.b200rl_synth_env_step(ptr(actions), ptr(obs), ptr(rewards), ptr(dones), ptr(time_outs), ptr(ep_t), N, D, A,
                                     max_len, p_done, seed, ptr(rng_epoch), step_index, _stream()), 'synth_env_step')
