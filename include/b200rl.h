@@ -524,6 +524,59 @@ int b200rl_synth_env_step(const float* actions, float* obs, float* rewards, uint
 int b200rl_bump_u64(uint64_t* p, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Soft Actor-Critic (sac_agent.py; csrc/sac.cu).  The MLP GEMMs are b200rl_linear_*; the optimiser steps b200rl_adam_step_f32.
+ * Random draws are Philox keyed by (seed, call site): the row is the low counter word, the device u64 *rng_ctr the high one
+ * (bump it with b200rl_bump_u64 between updates / env steps).  Call sites: 0 = next-action noise (critic target), 1 = actor noise,
+ * 2 = replay indices, 3 = rollout action noise, 4 = warmup uniform actions.
+ *  replay_insert: one env step of N rows into the ring (capacity >= N).  rb_state int64[2] = (head, fill), device-resident.
+ *                 terminated = done & !truncated, truncated = value_bootstrap & time_outs (time_outs may be NULL).
+ *                 next_step != 0: rows with prev_dones[r] set are skipped and the live rows keep their order; else at a truncated
+ *                 row next_obs is replaced by final_obs[r] (NULL: by obs[r]).  prev_dones (u8[N]) <- dones.  ep_state float[2N]
+ *                 = (current_rewards, current_lengths); meter double[3] = (mean reward, mean length, size) of AverageMeter.
+ *                 slot int[N], term_scratch / trunc_scratch u8[N]: work areas.
+ *  replay_sample: B rows at idx_tape[b] (NULL: uniform over the fill), obs normalised on read when norm_mean / norm_std are given
+ *                 (clamp to [-5, 5]).  x_cur = [obs | action], x_pi = [obs | (unwritten)], x_next = [next_obs | (unwritten)],
+ *                 all [B, D + A]; reward / not_done float[B]; idx_out (optional) int64[B].
+ *  squash_fwd:    head [M, 2A] = (mu, raw log_std) -> bounded log_std, x = mu + eps * std (eps from noise [M, A] or Philox),
+ *                 y = tanh(x); dst[r * dst_ld + j] = clamp(y * scale + bias, low, high) (optional); eps_out (optional);
+ *                 logp[r] = sum_j log N(x; mu, std) - 2 (log 2 - x - softplus(-2x)) - log_action_scale_sum (optional).
+ *  critic_loss:   stats[0..2] = (0.5 (l1 + l2), l1, l2); dq1 / dq2 = dL/dQ.
+ *  actor_loss:    stats[3] = actor loss, stats[4] = entropy, stats[6] = alpha loss; dq1 / dq2 = dL/dQ (ties split in halves);
+ *                 d_log_alpha[0] = alpha * mean(-logp - target_entropy) when learnable_temperature.
+ *  squash_bwd:    d_head [M, 2A] from dL/d(action) = dxa1 + dxa2 (rows of dx_ld floats) and max(alpha, min_alpha) / M * dlogp.
+ *  polyak:        target = lerp(target, src, tau); alpha_stat[0] = exp(log_alpha) when alpha_stat is given.
+ * ------------------------------------------------------------------------------------------- */
+int b200rl_sac_replay_insert_f32(const float* obs, const float* action, const float* reward, const float* next_obs,
+                                 const float* final_obs, const uint8_t* dones, const uint8_t* time_outs, int value_bootstrap,
+                                 int next_step, uint8_t* prev_dones, int N, int D, int A, int capacity, float* rb_obs,
+                                 float* rb_act, float* rb_rew, float* rb_next, uint8_t* rb_term, uint8_t* rb_trunc,
+                                 int64_t* rb_state, int* slot, uint8_t* term_scratch, uint8_t* trunc_scratch,
+                                 float* ep_state, double* meter, int games_to_track, void* stream);
+int b200rl_sac_replay_sample_f32(const float* rb_obs, const float* rb_act, const float* rb_rew, const float* rb_next,
+                                 const uint8_t* rb_term, const int64_t* rb_state, int capacity, int D, int A, int B,
+                                 const int64_t* idx_tape, uint64_t seed, const uint64_t* rng_ctr, const float* norm_mean,
+                                 const float* norm_std, float* x_cur, float* x_pi, float* x_next, float* reward,
+                                 float* not_done, int64_t* idx_out, void* stream);
+int b200rl_sac_squash_fwd_f32(const float* head, int M, int A, float log_std_min, float log_std_max, const float* noise,
+                              uint64_t seed, const uint64_t* rng_ctr, int rng_site, const float* act_scale,
+                              const float* act_bias, const float* act_low, const float* act_high, float log_action_scale_sum,
+                              float* dst, int64_t dst_ld, float* eps_out, float* logp, void* stream);
+int b200rl_sac_uniform_actions_f32(const float* act_low, const float* act_high, const float* u_tape, uint64_t seed,
+                                   const uint64_t* rng_ctr, float* out, int N, int A, void* stream);
+int b200rl_sac_critic_loss_f32(const float* q1, const float* q2, const float* q1t, const float* q2t, const float* logp_next,
+                               const float* reward, const float* not_done, const float* log_alpha, float gamma, int B,
+                               float* dq1, float* dq2, float* stats, void* stream);
+int b200rl_sac_actor_loss_f32(const float* q1, const float* q2, const float* logp, const float* log_alpha, float min_alpha,
+                              float target_entropy, int learnable_temperature, int B, float* dq1, float* dq2,
+                              float* d_log_alpha, float* stats, void* stream);
+int b200rl_sac_squash_bwd_f32(const float* head, const float* eps, int M, int A, float log_std_min, float log_std_max,
+                              const float* act_scale, const float* act_bias, const float* act_low, const float* act_high,
+                              const float* dxa1, const float* dxa2, int64_t dx_ld, const float* log_alpha, float min_alpha,
+                              float* d_head, void* stream);
+int b200rl_sac_polyak_f32(float* target, const float* src, int n, float tau, const float* log_alpha, float* alpha_stat,
+                          void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * bf16 tensor-core MLP path (`mixed_precision: True`, the reference's default on bf16-capable GPUs:
  * a2c_common.py:429, a2c_continuous.py:173).  wgmma chains + a per-CTA fp32 accumulator buffer in L2 + cp.async.bulk tile moves.
  * Network geometry supported by this build: MLP [256,128,64], A <= 15, and either obs dim <= 64 (BASELINE configs[1..2]: all

@@ -8,3 +8,9 @@ def register(runner):
     (imported lazily: the package itself stays importable without torch / the built library)"""
     from .runner import register as _register
     return _register(runner)
+
+
+def register_sac(runner):
+    """rl_games_b200.runner.register_sac: the B200 SAC agent behind `sac` in the given runner's algo_factory"""
+    from .runner import register_sac as _register_sac
+    return _register_sac(runner)

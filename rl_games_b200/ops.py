@@ -661,3 +661,62 @@ def value_loss(values, value_ld, old_values_n, returns_n, mask, rows_per_chunk, 
                                     float(e_clip), int(clip_value), ptr(inv_count), ptr(d_value), dv_ld, ptr(partials), partials.shape[0],
                                     ctypes.addressof(nb), _stream()), 'value_loss')
     return nb.value
+
+
+# ------------------------------------------------------------------------------------------ SAC (csrc/sac.cu)
+SAC_SITE_NEXT, SAC_SITE_ACTOR, SAC_SITE_REPLAY, SAC_SITE_ROLLOUT, SAC_SITE_WARMUP = 0, 1, 2, 3, 4     # Philox call sites (b200rl.h)
+
+
+def sac_replay_insert(obs, action, reward, next_obs, final_obs, dones_u8, time_outs_u8, value_bootstrap, next_step, prev_dones_u8, rb,
+                      slot, term_scratch, trunc_scratch, ep_state, meter, games_to_track):
+    """one env step into the ring buffer rb (dict: obs, act, rew, next, term, trunc, state); see include/b200rl.h"""
+    N, D = obs.shape
+    A = action.shape[1]
+    check(lib.b200rl_sac_replay_insert_f32(ptr(obs), ptr(action), ptr(reward), ptr(next_obs), ptr(final_obs), ptr(dones_u8), ptr(time_outs_u8),
+                                           int(bool(value_bootstrap)), int(bool(next_step)), ptr(prev_dones_u8), N, D, A, rb['obs'].shape[0],
+                                           ptr(rb['obs']), ptr(rb['act']), ptr(rb['rew']), ptr(rb['next']), ptr(rb['term']), ptr(rb['trunc']),
+                                           ptr(rb['state']), ptr(slot), ptr(term_scratch), ptr(trunc_scratch), ptr(ep_state), ptr(meter),
+                                           int(games_to_track), _stream()), 'sac_replay_insert')
+
+
+def sac_replay_sample(rb, B, idx_tape, seed, rng_ctr, norm_mean, norm_std, x_cur, x_pi, x_next, reward, not_done, idx_out=None):
+    D, A = rb['obs'].shape[1], rb['act'].shape[1]
+    check(lib.b200rl_sac_replay_sample_f32(ptr(rb['obs']), ptr(rb['act']), ptr(rb['rew']), ptr(rb['next']), ptr(rb['term']), ptr(rb['state']),
+                                           rb['obs'].shape[0], D, A, B, ptr(idx_tape), int(seed), ptr(rng_ctr), ptr(norm_mean), ptr(norm_std),
+                                           ptr(x_cur), ptr(x_pi), ptr(x_next), ptr(reward), ptr(not_done), ptr(idx_out), _stream()),
+          'sac_replay_sample')
+
+
+def sac_squash_fwd(head, M, A, log_std_bounds, noise, seed, rng_ctr, site, act, log_action_scale_sum, dst=None, dst_ld=0, eps_out=None,
+                   logp=None):
+    """act: (scale, bias, low, high) device tensors [A]"""
+    sc, bi, lo, hi = act
+    check(lib.b200rl_sac_squash_fwd_f32(ptr(head), M, A, float(log_std_bounds[0]), float(log_std_bounds[1]), ptr(noise), int(seed), ptr(rng_ctr),
+                                        int(site), ptr(sc), ptr(bi), ptr(lo), ptr(hi), float(log_action_scale_sum), ptr(dst), int(dst_ld),
+                                        ptr(eps_out), ptr(logp), _stream()), 'sac_squash_fwd')
+
+
+def sac_uniform_actions(low, high, u_tape, seed, rng_ctr, out, N, A):
+    check(lib.b200rl_sac_uniform_actions_f32(ptr(low), ptr(high), ptr(u_tape), int(seed), ptr(rng_ctr), ptr(out), N, A, _stream()),
+          'sac_uniform_actions')
+
+
+def sac_critic_loss(q1, q2, q1t, q2t, logp_next, reward, not_done, log_alpha, gamma, B, dq1, dq2, stats):
+    check(lib.b200rl_sac_critic_loss_f32(ptr(q1), ptr(q2), ptr(q1t), ptr(q2t), ptr(logp_next), ptr(reward), ptr(not_done), ptr(log_alpha),
+                                         float(gamma), B, ptr(dq1), ptr(dq2), ptr(stats), _stream()), 'sac_critic_loss')
+
+
+def sac_actor_loss(q1, q2, logp, log_alpha, min_alpha, target_entropy, learnable, B, dq1, dq2, d_log_alpha, stats):
+    check(lib.b200rl_sac_actor_loss_f32(ptr(q1), ptr(q2), ptr(logp), ptr(log_alpha), float(min_alpha), float(target_entropy), int(bool(learnable)),
+                                        B, ptr(dq1), ptr(dq2), ptr(d_log_alpha), ptr(stats), _stream()), 'sac_actor_loss')
+
+
+def sac_squash_bwd(head, eps, M, A, log_std_bounds, act, dxa1, dxa2, dx_ld, log_alpha, min_alpha, d_head):
+    sc, bi, lo, hi = act
+    check(lib.b200rl_sac_squash_bwd_f32(ptr(head), ptr(eps), M, A, float(log_std_bounds[0]), float(log_std_bounds[1]), ptr(sc), ptr(bi), ptr(lo),
+                                        ptr(hi), ptr(dxa1), ptr(dxa2), int(dx_ld), ptr(log_alpha), float(min_alpha), ptr(d_head), _stream()),
+          'sac_squash_bwd')
+
+
+def sac_polyak(target, src, tau, log_alpha=None, alpha_stat=None):
+    check(lib.b200rl_sac_polyak_f32(ptr(target), ptr(src), target.numel(), float(tau), ptr(log_alpha), ptr(alpha_stat), _stream()), 'sac_polyak')

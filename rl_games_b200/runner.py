@@ -62,6 +62,12 @@ def discrete_agent(**kwargs):
     return DiscreteA2CAgent(**kwargs)
 
 
+def sac_agent(**kwargs):
+    """Builder for the algo name `sac` (sac_agent.py)"""
+    from .agent_sac import SACAgent
+    return SACAgent(**kwargs)
+
+
 _continuous_agent, _discrete_agent = continuous_agent, discrete_agent
 
 
@@ -70,6 +76,12 @@ def register(runner):
     `rl_games.torch_runner.Runner` (torch_runner.py:117-120) or this module's mirror -- so that stock YAMLs run unchanged."""
     runner.algo_factory.register_builder('a2c_continuous', lambda **kwargs: continuous_agent(**kwargs))
     runner.algo_factory.register_builder('a2c_discrete', lambda **kwargs: discrete_agent(**kwargs))
+    return runner
+
+
+def register_sac(runner):
+    """Put the B200 SAC agent behind the reference's algo name `sac` in any runner with an `algo_factory` ObjectFactory"""
+    runner.algo_factory.register_builder('sac', lambda **kwargs: sac_agent(**kwargs))
     return runner
 
 
@@ -109,6 +121,8 @@ class Runner:
         print(f'self.seed = {self.seed}')
         self.algo_params = params['algo']
         self.algo_name = self.algo_params['name']
+        if self.algo_name == 'sac':
+            register_sac(self)
         self.exp_config = None
         if self.seed:
             torch.manual_seed(self.seed)
