@@ -180,9 +180,12 @@ int b200rl_reduce_splits_f32(const float* part, float* out, int n, int n_splits,
  *  cell_fwd: gates [S,4Hd] pre-activations -> activations in place; cin = already-masked c_{t-1}; writes c_out, h_out,
  *            optionally scatters h into an MLP-order buffer (row s -> (s/scatter_rpc)*scatter_stride + s%scatter_rpc) and the
  *            masked carries (h,c)*(1-done_next) for the next step (done_next rows chunk-mapped).
- *  cell_bwd: dh = dH[scatter row] + dhin_next*(1-done_next), dc = dcin_next*(1-done_next) -> dgates [S,4Hd], dcin [S,Hd].
+ *  cell_bwd: dh = dH[scatter row] + dhin_next*(1-done_next), dc = dcin_next*(1-done_next) -> dgates [S,4Hd], dcin [S,Hd]
+ *            (dH needs scatter_rpc > 0: scatter_rpc = S, scatter_stride = 0 for dense rows).
  *  mask_rows: out[s] = in[chunk row s] * (1 - done[chunk row s])  (window-initial states; zeroing after episode ends,
  *             a2c_common.py:1150-1153)
+ *  A row mapping of zero rows per chunk (scatter_rpc with h_scatter / dH, done_rpc with done_next / done, in_rpc) is refused with
+ *  B200RL_EINVAL before anything is written.
  * ------------------------------------------------------------------------------------------- */
 int b200rl_lstm_cell_fwd_f32(float* gates, const float* cin, float* c_out, float* h_out, float* h_scatter, int scatter_rpc,
                              int64_t scatter_stride, float* hin_next, float* cin_next, const uint8_t* done_next,

@@ -238,6 +238,8 @@ B200RL_EXPORT int b200rl_lstm_cell_bwd_f32(const float* gates_act, const float* 
                                            int done_rpc, int64_t done_stride, float* dgates, float* dcin, int S, int Hd, void* stream) {
     if (!gates_act || !c_t || !cin || !dgates || !dcin || S <= 0 || Hd <= 0) return B200RL_EINVAL;
     if ((dhin_next == nullptr) != (dcin_next == nullptr)) return B200RL_EINVAL;
+    if (dH && scatter_rpc <= 0) return B200RL_EINVAL;          // a dH without its row mapping would read row 0 for every row
+    if (done_next && done_rpc <= 0) return B200RL_EINVAL;
     const int64_t n = (int64_t)S * Hd;
     lstm_cell_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, as_stream(stream)>>>(gates_act, c_t, cin, dH, scatter_rpc > 0 ? scatter_rpc : 1,
                                                                                      scatter_stride, dhin_next, dcin_next, done_next,
@@ -249,6 +251,7 @@ B200RL_EXPORT int b200rl_lstm_cell_bwd_f32(const float* gates_act, const float* 
 B200RL_EXPORT int b200rl_rnn_mask_rows_f32(const float* in, int in_rpc, int64_t in_stride, float* out, const uint8_t* done, int done_rpc,
                                            int64_t done_stride, int S, int Hd, void* stream) {
     if (!in || !out || S <= 0 || Hd <= 0 || in_rpc <= 0) return B200RL_EINVAL;
+    if (done && done_rpc <= 0) return B200RL_EINVAL;           // a done vector without its row mapping would read done[0] for every row
     const int64_t n = (int64_t)S * Hd;
     rnn_mask_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, as_stream(stream)>>>(in, in_rpc, in_stride, out, done, done_rpc > 0 ? done_rpc : 1,
                                                                                      done_stride, S, Hd);
