@@ -26,10 +26,10 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import ops
+from . import layerwise, ops
 from .a2c_base import A2CBase
 from .common import IdentityScheduler
-from .model import B200Model
+from .model import B200Model, _RunningStats
 
 STATS_SYNC_MODES = ('pooled', 'broadcast')
 
@@ -139,9 +139,9 @@ class A2CAgent(A2CBase):
         # BPTT), MLPs wider / deeper than the fused tiles.  The reference's autocast covers nn.LSTM and nn.Linear alike (a2c_continuous.py:173).
         self.use_tc = bool(self.mixed_precision) and fused_ok
         self.gemm_tc = bool(self.mixed_precision) and not fused_ok
-        self._lin_fwd = ops.linear_fwd_tc if self.gemm_tc else ops.linear_fwd
-        self._lin_bwd = ops.linear_bwd_data_tc if self.gemm_tc else ops.linear_bwd_data
-        self._lin_bww = ops.linear_bwd_weight_tc if self.gemm_tc else ops.linear_bwd_weight
+        self.obs_norm = _RunningStats.f32_pair(self.model.running_mean_std)
+        # with an LSTM in front the MLP input is h (dense, not normalised)
+        self.mlp_norm = (None, None) if (self.is_rnn and self.model.rnn_before_mlp) else self.obs_norm
         self.tc_wide = self.use_tc and ops.tc_kind(self.model.D, self.model.units, self.actions_num) == 2
         # Rollout precision.  The reference evaluates the policy during the rollout OUTSIDE autocast (a2c_common.py:581-600: fp32 / TF32)
         # and only calc_gradients under bf16 autocast (a2c_continuous.py:173).  Default here: the rollout uses the same bf16 wgmma
@@ -279,12 +279,10 @@ class A2CAgent(A2CBase):
             # c4 gate GEMM (16 tiles) at 256 CTAs while the split partials stay small (64 splits: 91 MB of partials per gate GEMM)
             self.n_splits = max(1, min(16, mb // 512))
             self.wbf = torch.empty(m.num_params, dtype=torch.bfloat16, device=dev)     # bf16 twin of the parameter arena (weight operands)
-            import functools
-            arena = (m.flat, self.wbf)
-            self._lin_fwd = functools.partial(ops.linear_fwd_tc, bf16_arena=arena)
-            self._lin_bwd = functools.partial(ops.linear_bwd_data_tc, bf16_arena=arena)
         else:
-            self.n_splits = max(1, min(64, mb // 256))
+            self.n_splits = layerwise.n_splits(mb)
+        # the layer-wise GEMMs: MLP (fp32 path, layer-wise tensor-core path, fp32 rollout of the fused path), LSTM gates, head gradient
+        self.kernels = layerwise.Kernels(tc=self.gemm_tc, bf16_arena=(m.flat, self.wbf) if self.gemm_tc else None)
         self.part_rows = self.n_splits * (self.seq_length if self.is_rnn else 1)
         # split-partial gradient rows; the wgmma path pads the row stride to 16 bytes so the reduction can use float4 loads
         self.part = f(self.part_rows, (m.num_params + 3) // 4 * 4 if self.use_tc else m.num_params)
@@ -309,10 +307,7 @@ class A2CAgent(A2CBase):
         # comm buffer = flat gradient + 1 KL slot (one all-reduce per minibatch, a2c_common.py:493-509 + :1559-1561)
         self.comm = f(m.num_params + 1)
         m.grad = self.comm[:m.num_params]
-        m.gW = [m.view(f'W{i}', m.grad) for i in range(len(m.units))]
-        m.gb = [m.view(f'b{i}', m.grad) for i in range(len(m.units))]
         m.g_sigma = m.view('sigma', m.grad)
-        m.gW_head, m.gb_head = m.view('W_head', m.grad), m.view('b_head', m.grad)
         self.kl_slot = self.comm[m.num_params:]
         self._gv = [dict(grad=m.grad, g_sigma=m.g_sigma, kl=self.kl_slot, comm=self.comm)] * 2
         self.fused_allreduce = False
@@ -538,13 +533,7 @@ class A2CAgent(A2CBase):
 
     # =============================================================================== policy forward
     def _trunk(self, x, acts, M, rows_per_chunk=None, chunk_stride=0):
-        m = self.model
-        # with an LSTM in front the MLP input is h (dense, not normalised)
-        nm, ns = (None, None) if (self.is_rnn and m.rnn_before_mlp) else self._norm()
-        self._lin_fwd(x, m.W[0], m.b[0], acts[0], m.act_id, rows_per_chunk=rows_per_chunk, chunk_stride=chunk_stride,
-                       x_ld=m.mlp_in, norm_mean=nm, norm_std=ns, M=M)
-        for i in range(1, len(m.units)):
-            self._lin_fwd(acts[i - 1], m.W[i], m.b[i], acts[i], m.act_id, M=M)
+        layerwise.forward(self.kernels, self.model.mlp, x, acts, M, self.model.mlp_in, rows_per_chunk, chunk_stride, self.mlp_norm)
 
     def _repack(self):
         """bf16 operand copy of the weights for the wgmma kernels (after every optimiser step / weight load)."""
@@ -554,17 +543,13 @@ class A2CAgent(A2CBase):
         if getattr(self, 'gemm_tc', False) and self._tensors_ready:
             ops.cast_bf16(self.model.flat, self.wbf)
 
-    def _norm(self):
-        m = self.model
-        return (m.running_mean_std.mean_f32, m.running_mean_std.std_f32) if self.normalize_input else (None, None)
-
     def _lstm_step(self, obs, h_in, c_in, h_out, c_out):
         """one LSTM step for all N envs (seq_length 1, models.py -> network_builder.py:452-492 -> recurrent.py): returns h_out, or its
         LayerNorm (in self.r_y) with rnn.layer_norm"""
         m, N = self.model, self.num_rows
-        nm, ns = self._norm() if m.rnn_before_mlp else (None, None)      # after the MLP the LSTM reads the trunk output
-        self._lin_fwd(obs, m.W_ih, m.b_ih, self.r_gates, 0, x_ld=m.rnn_in, norm_mean=nm, norm_std=ns, M=N)
-        self._lin_fwd(h_in, m.W_hh, m.b_hh, self.r_gates, 0, M=N, accumulate=True)
+        nm, ns = self.obs_norm if m.rnn_before_mlp else (None, None)      # after the MLP the LSTM reads the trunk output
+        self.kernels.fwd(obs, m.W_ih, m.b_ih, self.r_gates, 0, x_ld=m.rnn_in, norm_mean=nm, norm_std=ns, M=N)
+        self.kernels.fwd(h_in, m.W_hh, m.b_hh, self.r_gates, 0, M=N, accumulate=True)
         if m.rnn_layer_norm:     # the trunk / heads read LayerNorm(h); h_out / c_out stay the raw carried states
             ops.lstm_cell_ln_fwd(self.r_gates, c_in, c_out, h_out, m.ln_w, m.ln_b, N, m.rnn_units, y_out=self.r_y)
             return self.r_y
@@ -574,7 +559,7 @@ class A2CAgent(A2CBase):
     def _policy_step(self, obs, t, noise=None):
         m, N, A = self.model, self.num_rows, self.actions_num
         if self.use_tc and not self.rollout_fp32:
-            nm, ns = self._norm()
+            nm, ns = self.obs_norm
             ops.tc_mlp_fwd_rollout(obs, m.D, nm, ns, self.wpack, m.b, m.b_head, m.sigma, m.units, N, A,
                                    m.value_mean_std.running_mean, m.value_mean_std.running_var, self.normalize_value, noise,
                                    self.rng_seed, self.rng_epoch, t, self.actions[t], self.mus[t], self.sigmas[t],
@@ -608,7 +593,7 @@ class A2CAgent(A2CBase):
         o = obs['obs'] if isinstance(obs, dict) else obs
         m, N, A = self.model, self.num_rows, self.actions_num
         if self.use_tc and not self.rollout_fp32:
-            nm, ns = self._norm()
+            nm, ns = self.obs_norm
             ops.tc_mlp_fwd_rollout(o, m.D, nm, ns, self.wpack, m.b, m.b_head, m.sigma, m.units, N, A,
                                    m.value_mean_std.running_mean, m.value_mean_std.running_var, self.normalize_value, None, 0, None,
                                    0, None, None, None, None, self.last_values, None, False, None, None, None, None, None, None,
@@ -753,7 +738,6 @@ class A2CAgent(A2CBase):
         epm, mb = self.envs_per_mb, self.minibatch_size
         e0 = i * epm
         x = self.obses[0, e0:]
-        L = len(m.units)
         if self.normalize_input:
             rms = m.running_mean_std
             if self.use_mb_moments:
@@ -801,28 +785,15 @@ class A2CAgent(A2CBase):
         S = min(self.part_rows, max(self.n_splits, mb // 256)) if self.gemm_tc else self.n_splits
         off_wh, _ = m.layout['W_head']
         off_bh, _ = m.layout['b_head']
-        self._lin_bww(self.d_head, a_last, self.part[0, off_wh:], self.part[0, off_bh:], m.Hl, m.head_rows, S, M=mb,
-                              split_stride=P)
+        self.kernels.bwd_weight(self.d_head, a_last, self.part[0, off_wh:], self.part[0, off_bh:], m.Hl, m.head_rows, S, M=mb,
+                                split_stride=P)
         if rnn_last:
             self._lstm_window_bwd(e0)       # also fills dA[-1] = dL/d(pre-activation of the last MLP layer)
-        nm = m.running_mean_std.mean_f32 if self.normalize_input else None
-        ns = m.running_mean_std.std_f32 if self.normalize_input else None
-        for l in range(L - 1, -1, -1):
-            off_w, shp = m.layout[f'W{l}']
-            off_b, _ = m.layout[f'b{l}']
-            if l > 0:
-                self._lin_bww(self.dA[l], self.ta[l - 1], self.part[0, off_w:], self.part[0, off_b:], shp[1], shp[0], S,
-                                      M=mb, split_stride=P)
-                self._lin_bwd(self.dA[l], m.W[l], self.ta[l - 1], self.dA[l - 1], m.act_id, M=mb)
-            elif rnn_first:
-                self._lin_bww(self.dA[0], self.t_hmlp, self.part[0, off_w:], self.part[0, off_b:], shp[1], shp[0], S, M=mb,
-                                      split_stride=P)
-                self._lin_bwd(self.dA[0], m.W[0], None, self.t_dHmlp, 0, M=mb)
-                self._lstm_window_bwd(e0)
-            else:
-                self._lin_bww(self.dA[0], x, self.part[0, off_w:], self.part[0, off_b:], shp[1], shp[0], S,
-                                      rows_per_chunk=epm, chunk_stride=N, x_ld=m.D, norm_mean=nm, norm_std=ns, M=mb,
-                                      split_stride=P)
+        if rnn_first:       # the MLP hands dL/dh back to the LSTM
+            layerwise.backward(self.kernels, m.mlp, self.t_hmlp, self.ta, self.dA, self.part, P, S, mb, m.mlp_in, dx_out=self.t_dHmlp)
+            self._lstm_window_bwd(e0)
+        else:
+            layerwise.backward(self.kernels, m.mlp, x, self.ta, self.dA, self.part, P, S, mb, m.D, epm, N, self.mlp_norm)
         ops.reduce_splits(self.part[0, A:], gv['grad'][A:], P - A, self.part_rows, split_stride=P)
         if m.grad_mask is not None:      # separate trunks: the structural zeros of the block layout get no gradient (model.py)
             gv['grad'][:P].mul_(m.grad_mask)
@@ -835,7 +806,7 @@ class A2CAgent(A2CBase):
         m, H, N, T = self.model, self.horizon_length, self.num_rows, self.seq_length
         epm, Hd = self.envs_per_mb, m.rnn_units
         S = epm * H // T
-        nm, ns = self._norm() if m.rnn_before_mlp else (None, None)
+        nm, ns = self.obs_norm if m.rnn_before_mlp else (None, None)
         # window-initial states = snapshots taken during the rollout, zeroed where the episode ended entering step 0
         dn = self.rnn_dones_buf if self.rnn_dones_buf is not None else self.dones_buf
         ops.rnn_mask_rows(self.rnn_h0[0, e0:], epm, N, self.t_hin[0], S, Hd, done=dn[0, e0:], done_rpc=epm, done_stride=T * N)
@@ -843,9 +814,9 @@ class A2CAgent(A2CBase):
         for t in range(T):
             # step-t inputs of all S sequences: arena observations (LSTM first) or the trunk output rows (j*T + t)*epm + e (LSTM last)
             xin, xstride = (self.obses[t, e0:], T * N) if m.rnn_before_mlp else (self.ta[-1][t * epm:], T * epm)
-            self._lin_fwd(xin, m.W_ih, m.b_ih, self.t_gates[t], 0, rows_per_chunk=epm, chunk_stride=xstride, x_ld=m.rnn_in,
-                           norm_mean=nm, norm_std=ns, M=S)
-            self._lin_fwd(self.t_hin[t], m.W_hh, m.b_hh, self.t_gates[t], 0, M=S, accumulate=True)
+            self.kernels.fwd(xin, m.W_ih, m.b_ih, self.t_gates[t], 0, rows_per_chunk=epm, chunk_stride=xstride, x_ld=m.rnn_in,
+                             norm_mean=nm, norm_std=ns, M=S)
+            self.kernels.fwd(self.t_hin[t], m.W_hh, m.b_hh, self.t_gates[t], 0, M=S, accumulate=True)
             last = t == T - 1
             if m.rnn_layer_norm:     # the MLP-order rows get LayerNorm(h); the carries stay raw; mean / rstd kept for the backward
                 ops.lstm_cell_ln_fwd(self.t_gates[t], self.t_cin[t], self.t_c[t], self.t_hdense, m.ln_w, m.ln_b, S, Hd,
@@ -865,8 +836,9 @@ class A2CAgent(A2CBase):
         m, H, N, T = self.model, self.horizon_length, self.num_rows, self.seq_length
         epm, Hd, P, Ssp = self.envs_per_mb, m.rnn_units, m.num_params, self.n_splits
         S = epm * H // T
-        nm, ns = self._norm() if m.rnn_before_mlp else (None, None)
-        o_wih, o_whh, o_bih, o_bhh = (m.layout[k][0] for k in ('W_ih', 'W_hh', 'b_ih', 'b_hh'))
+        nm, ns = self.obs_norm if m.rnn_before_mlp else (None, None)
+        k = self.kernels
+        o_wih, o_whh, o_bih, o_bhh = (m.layout[n][0] for n in ('W_ih', 'W_hh', 'b_ih', 'b_hh'))
         dn = self.rnn_dones_buf if self.rnn_dones_buf is not None else self.dones_buf
         for t in range(T - 1, -1, -1):
             last = t == T - 1
@@ -885,24 +857,24 @@ class A2CAgent(A2CBase):
                                   dhin_next=None if last else self.t_dhin, dcin_next=None if last else self.t_dcin[(t + 1) & 1],
                                   done_next=None if last else dn[t + 1, e0:], done_rpc=epm, done_stride=T * N)
             xin, xstride = (self.obses[t, e0:], T * N) if m.rnn_before_mlp else (self.ta[-1][t * epm:], T * epm)
-            self._lin_bww(self.t_dgates, xin, self.part[row, o_wih:], self.part[row, o_bih:], m.rnn_in, 4 * Hd, Ssp,
-                                  rows_per_chunk=epm, chunk_stride=xstride, x_ld=m.rnn_in, norm_mean=nm, norm_std=ns, M=S, split_stride=P)
-            self._lin_bww(self.t_dgates, self.t_hin[t], self.part[row, o_whh:], self.part[row, o_bhh:], Hd, 4 * Hd, Ssp, M=S,
-                                  split_stride=P)
+            k.bwd_weight(self.t_dgates, xin, self.part[row, o_wih:], self.part[row, o_bih:], m.rnn_in, 4 * Hd, Ssp,
+                         rows_per_chunk=epm, chunk_stride=xstride, x_ld=m.rnn_in, norm_mean=nm, norm_std=ns, M=S, split_stride=P)
+            k.bwd_weight(self.t_dgates, self.t_hin[t], self.part[row, o_whh:], self.part[row, o_bhh:], Hd, 4 * Hd, Ssp, M=S,
+                         split_stride=P)
             if t > 0:
-                self._lin_bwd(self.t_dgates, m.W_hh, None, self.t_dhin, 0, M=S)
+                k.bwd_data(self.t_dgates, m.W_hh, None, self.t_dhin, 0, M=S)
             if not m.rnn_before_mlp:
                 # dgrad through W_ih into the trunk: sequences j*epm..(j+1)*epm-1 at step t are trunk rows (j*T + t)*epm.., one dense
                 # epm-row block each; the last MLP layer's activation derivative is folded in (dA[-1] is d pre-activation)
                 for j in range(H // T):
                     r0 = (j * T + t) * epm
-                    self._lin_bwd(self.t_dgates[j * epm:], m.W_ih, self.ta[-1][r0:], self.dA[-1][r0:], m.act_id, M=epm)
+                    k.bwd_data(self.t_dgates[j * epm:], m.W_ih, self.ta[-1][r0:], self.dA[-1][r0:], m.act_id, M=epm)
 
     def _minibatch_update_tc(self, i, u, x, e0):
         """bf16 wgmma edition: fused fwd+loss kernel, two backward kernels, split reduce, Adam, repack."""
         m, H, N, A = self.model, self.horizon_length, self.num_rows, self.actions_num
         epm, mb, P = self.envs_per_mb, self.minibatch_size, self.model.num_params
-        nm, ns = self._norm()
+        nm, ns = self.obs_norm
         nb = ops.tc_mlp_fwd_train(x, epm, N, m.D, nm, ns, self.wpack, m.b, m.b_head, m.sigma, m.units, mb, A, self.actions[0, e0:],
                                   self.mus[0, e0:], self.sigmas[0, e0:], self.old_values_n[0, e0:], self.returns_n[0, e0:],
                                   self.neglogpacs[0, e0:], self.advs_n[0, e0:], None if self.valid is None else self.valid[0, e0:],

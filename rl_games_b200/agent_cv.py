@@ -21,9 +21,10 @@ from collections import OrderedDict
 import torch
 import torch.distributed as dist
 
-from . import ops
+from . import layerwise, ops
 from .agent import A2CAgent
 from .common import IdentityScheduler, LinearScheduler
+from .layerwise import Layer
 from .model import FlatParamModel, _RunningStats, check_network_params
 
 
@@ -95,14 +96,17 @@ class CentralValueNet(FlatParamModel):
         self._init_linear_default()
         self.running_mean_std = _RunningStats(self.S, dev) if self.normalize_input else None
         self.value_mean_std = _RunningStats(1, dev) if self.normalize_value else None
+        self.obs_norm = _RunningStats.f32_pair(self.running_mean_std)
+        # the value layer is the MLP's linear output layer
+        names = [(f'W{i}', f'b{i}', self.act_id) for i in range(len(self.units))] + [('W_v', 'b_v', 0)]
+        self.mlp = [Layer(self.view(w), self.view(b), self.layout[w][0], self.layout[b][0], act) for w, b, act in names]
+        self.kernels = layerwise.Kernels()
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)   # noqa: E731
         mb = self.minibatch_size
         self.states = f(self.H, self.N, self.S)
-        self.r_act = [f(self.N, u) for u in self.units]
-        self.t_act = [f(mb, u) for u in self.units]
-        self.d_act = [f(mb, u) for u in self.units]
-        self.r_val, self.t_val, self.d_val = f(self.N, 1), f(mb, 1), f(mb, 1)
-        self.n_splits = max(1, min(64, mb // 256))
+        # activations (rollout, training) and their gradients; the last entry is the value
+        self.r_act, self.t_act, self.d_act = ([f(M, u) for u in self.units] + [f(M, 1)] for M in (self.N, mb, mb))
+        self.n_splits = layerwise.n_splits(mb)
         self.part = f(self.n_splits, off)
         self.grad = f(off)
         self.loss_partials = torch.zeros((mb + 255) // 256, 8, dtype=torch.float64, device=dev)
@@ -136,28 +140,20 @@ class CentralValueNet(FlatParamModel):
         super().load_state_dict({k[len('model.'):] if k.startswith('model.') else k: v for k, v in sd.items()}, strict)
 
     # ---------------------------------------------------------------------------------------------- forward
-    def _trunk(self, x, acts, M, rows_per_chunk=None, chunk_stride=0):
-        r = self.running_mean_std
-        nm, ns = (r.mean_f32, r.std_f32) if self.normalize_input else (None, None)
-        ops.linear_fwd(x, self.view('W0'), self.view('b0'), acts[0], self.act_id, rows_per_chunk=rows_per_chunk, chunk_stride=chunk_stride,
-                       x_ld=self.S, norm_mean=nm, norm_std=ns, M=M)
-        for i in range(1, len(self.units)):
-            ops.linear_fwd(acts[i - 1], self.view(f'W{i}'), self.view(f'b{i}'), acts[i], self.act_id, M=M)
-
     def get_value(self, states, out):
         """central_value.py:207-229 (eval mode): out[N] = denorm(critic(states)); with agents > 1, out[N * agents] = each env's value on
         each of its agent rows"""
-        self._trunk(states, self.r_act, self.N)
-        ops.linear_fwd(self.r_act[-1], self.view('W_v'), self.view('b_v'), self.r_val, 0, M=self.N)
+        layerwise.forward(self.kernels, self.mlp, states, self.r_act, self.N, self.S, norm=self.obs_norm)
+        val = self.r_act[-1]
         if self.agents > 1:
             vm = self.value_mean_std
-            ops.cv_value_broadcast(self.r_val, vm.running_mean if vm else None, vm.running_var if vm else None, self.normalize_value, out,
+            ops.cv_value_broadcast(val, vm.running_mean if vm else None, vm.running_var if vm else None, self.normalize_value, out,
                                    self.N, self.agents)
         elif self.normalize_value:
             vm = self.value_mean_std
-            ops.normalize(self.r_val, vm.running_mean, vm.running_var, denorm=True, out=out.view(self.N, 1))
+            ops.normalize(val, vm.running_mean, vm.running_var, denorm=True, out=out.view(self.N, 1))
         else:
-            out.copy_(self.r_val.view(-1))
+            out.copy_(val.view(-1))
 
     # ---------------------------------------------------------------------------------------------- training (central_value.py:246-274)
     def train_net(self, old_values_n, returns_n, valid):
@@ -179,28 +175,12 @@ class CentralValueNet(FlatParamModel):
                     r = self.running_mean_std
                     ops.moments_update(x, self.S, epm, H, N, r.running_mean, r.running_var, r.count, r.mean_f32, r.std_f32, self.mom_scratch,
                                        self.counters[1:2])
-                self._trunk(x, self.t_act, mb, rows_per_chunk=epm, chunk_stride=N)
-                ops.linear_fwd(self.t_act[-1], self.view('W_v'), self.view('b_v'), self.t_val, 0, M=mb)
-                nb = ops.value_loss(self.t_val, 1, old_values_n[0, e0:], returns_n[0, e0:], None if valid is None else valid[0, e0:], epm, N, mb,
-                                    self.e_clip, self.clip_value, None if valid is None else self.inv_counts[i:i + 1], self.d_val, 1,
+                layerwise.forward(self.kernels, self.mlp, x, self.t_act, mb, self.S, epm, N, self.obs_norm)
+                nb = ops.value_loss(self.t_act[-1], 1, old_values_n[0, e0:], returns_n[0, e0:], None if valid is None else valid[0, e0:], epm, N, mb,
+                                    self.e_clip, self.clip_value, None if valid is None else self.inv_counts[i:i + 1], self.d_act[-1], 1,
                                     self.loss_partials)
                 rows.append(self.loss_partials[:nb, 0].sum().float())
-                off_w, _ = self.layout['W_v']
-                off_b, _ = self.layout['b_v']
-                ops.linear_bwd_weight(self.d_val, self.t_act[-1], self.part[0, off_w:], self.part[0, off_b:], self.Hl, 1, S_, M=mb, split_stride=P)
-                ops.linear_bwd_data(self.d_val, self.view('W_v'), self.t_act[-1], self.d_act[-1], self.act_id, M=mb)
-                r = self.running_mean_std
-                nm, ns = (r.mean_f32, r.std_f32) if self.normalize_input else (None, None)
-                for l in range(len(self.units) - 1, -1, -1):
-                    off_w, shp = self.layout[f'W{l}']
-                    off_b, _ = self.layout[f'b{l}']
-                    if l > 0:
-                        ops.linear_bwd_weight(self.d_act[l], self.t_act[l - 1], self.part[0, off_w:], self.part[0, off_b:], shp[1], shp[0], S_,
-                                              M=mb, split_stride=P)
-                        ops.linear_bwd_data(self.d_act[l], self.view(f'W{l}'), self.t_act[l - 1], self.d_act[l - 1], self.act_id, M=mb)
-                    else:
-                        ops.linear_bwd_weight(self.d_act[0], x, self.part[0, off_w:], self.part[0, off_b:], shp[1], shp[0], S_,
-                                              rows_per_chunk=epm, chunk_stride=N, x_ld=self.S, norm_mean=nm, norm_std=ns, M=mb, split_stride=P)
+                layerwise.backward(self.kernels, self.mlp, x, self.t_act, self.d_act, self.part, P, S_, mb, self.S, epm, N, self.obs_norm)
                 ops.reduce_splits(self.part, self.grad, P, S_, split_stride=P)
                 if self.multi_gpu:      # the critic's own flat-gradient exchange, one per minibatch (central_value.py:322-337)
                     dist.all_reduce(self.grad, op=dist.ReduceOp.SUM)

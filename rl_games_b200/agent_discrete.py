@@ -20,9 +20,10 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import ops
+from . import layerwise, ops
 from .a2c_base import A2CBase
 from .common import make_summary_writer
+from .layerwise import Layer
 from .model import check_network_params, FlatParamModel, _RunningStats
 
 
@@ -66,10 +67,21 @@ class DiscreteModel(FlatParamModel):
         self._init_linear_default()          # network_builder.py:332-340 with the 'default' initializer
         self.running_mean_std = _RunningStats(self.D, self.device) if self.normalize_input else None
         self.value_mean_std = _RunningStats(1, self.device) if self.normalize_value else None
+        # the head is the linear output layer of the trunk's MLP: one MLP into [value | logits] when the trunk is shared; with separate
+        # trunks the actor MLP ends in the logit rows of the head, the critic MLP in its value row
+        wh, bh = self.view('W_head'), self.view('b_head')
+        off_wh, off_bh = self.layout['W_head'][0], self.layout['b_head'][0]
+        self.actor_mlp = self._trunk_layers('a')
+        if self.separate:
+            self.actor_mlp.append(Layer(wh[1:], bh[1:], off_wh + self.Hl, off_bh + 1, 0))
+            self.critic_mlp = self._trunk_layers('c') + [Layer(wh[:1], bh[:1], off_wh, off_bh, 0)]
+        else:
+            self.actor_mlp.append(Layer(wh, bh, off_wh, off_bh, 0))
+            self.critic_mlp = None
 
-    def trunk(self, which):
-        p = 'a' if which == 'actor' or not self.separate else 'c'
-        return [(self.view(f'W{p}{i}'), self.view(f'b{p}{i}')) for i in range(len(self.units))]
+    def _trunk_layers(self, p):
+        return [Layer(self.view(f'W{p}{i}'), self.view(f'b{p}{i}'), self.layout[f'W{p}{i}'][0], self.layout[f'b{p}{i}'][0], self.act_id)
+                for i in range(len(self.units))]
 
     def _param_views(self, arena=None):
         out = []
@@ -191,16 +203,18 @@ class DiscreteA2CAgent(A2CBase):
         self.prev_dones = f(N) if self.mask_autoreset_rows else None
         self.meter = torch.zeros(8, dtype=torch.float64, device=dev)
         self.rng_epoch = torch.zeros(1, dtype=torch.int64, device=dev)
-        L = len(m.units)
-        # rollout / training activations of the actor trunk (and the critic trunk when separate), head buffers
-        self.r_a = [f(N, u) for u in m.units]
-        self.r_c = [f(N, u) for u in m.units] if m.separate else self.r_a
-        self.t_a = [f(mb, u) for u in m.units]
-        self.t_c = [f(mb, u) for u in m.units] if m.separate else self.t_a
-        self.d_a = [f(mb, u) for u in m.units]
-        self.d_c = [f(mb, u) for u in m.units] if m.separate else self.d_a
-        self.r_head, self.t_head, self.d_head = f(N, 1 + K), f(mb, 1 + K), f(mb, 1 + K)
-        self.n_splits = max(1, min(64, mb // 256))
+        # activations of the actor MLP (and the critic MLP when separate), rollout (r_) and training (t_), and their gradients (d_); the
+        # last entry is the MLP's output layer: [value | logits] (shared trunk) or the logits / the value (separate trunks)
+        self.r_a, self.t_a, self.d_a = ([f(M, u) for u in m.units] + [f(M, K if m.separate else 1 + K)] for M in (N, mb, mb))
+        # (logits, ld, value, value ld) of the head output (rollout, training) and of its gradient
+        if m.separate:
+            self.r_c, self.t_c, self.d_c = ([f(M, u) for u in m.units] + [f(M, 1)] for M in (N, mb, mb))
+            self.r_out, self.t_out, self.d_out = ((a[-1], K, c[-1], 1) for a, c in ((self.r_a, self.r_c), (self.t_a, self.t_c),
+                                                                                    (self.d_a, self.d_c)))
+        else:
+            self.r_c = self.t_c = self.d_c = None
+            self.r_out, self.t_out, self.d_out = ((a[-1][:, 1:], K + 1, a[-1], K + 1) for a in (self.r_a, self.t_a, self.d_a))
+        self.n_splits = layerwise.n_splits(mb)
         self.part = f(self.n_splits, m.num_params)
         self.grad = f(m.num_params)
         self.diag_exp_var = f(self.num_minibatches) if self.diag_on else None
@@ -219,8 +233,9 @@ class DiscreteA2CAgent(A2CBase):
         rs = self.rewards_shaper
         self.shaper_cfg = ops.ShaperCfg(float(rs.scale_value), float(rs.shift_value), float(rs.min_val), float(rs.max_val),
                                         float(self.gamma), int(bool(rs.log_val)), int(bool(self.value_bootstrap)))
+        self.obs_norm = _RunningStats.f32_pair(m.running_mean_std)
+        self.kernels = layerwise.Kernels()
         self._tensors_ready = True
-        assert L >= 1
 
     # =============================================================================== env plumbing (tensor envs on the device)
     def _to_dev(self, x, dtype=None):
@@ -238,47 +253,13 @@ class DiscreteA2CAgent(A2CBase):
         o = o['obs'] if isinstance(o, dict) else o
         return self._to_dev(o, torch.float32).contiguous(), self._to_dev(rewards, torch.float32), self._to_dev(dones), infos
 
-    # =============================================================================== forward pieces
-    def _norm(self):
-        r = self.model.running_mean_std
-        return (r.mean_f32, r.std_f32) if self.normalize_input else (None, None)
-
-    def _trunk(self, layers, x, acts, M, rows_per_chunk=None, chunk_stride=0):
-        nm, ns = self._norm()
+    # =============================================================================== forward
+    def _forward(self, x, acts_a, acts_c, M, rows_per_chunk=None, chunk_stride=0):
+        """the actor MLP into acts_a (its last entry: [value | logits], or the logits with separate trunks), the critic MLP into acts_c"""
         m = self.model
-        ops.linear_fwd(x, layers[0][0], layers[0][1], acts[0], m.act_id, rows_per_chunk=rows_per_chunk, chunk_stride=chunk_stride,
-                       x_ld=m.D, norm_mean=nm, norm_std=ns, M=M)
-        for i in range(1, len(layers)):
-            ops.linear_fwd(acts[i - 1], layers[i][0], layers[i][1], acts[i], m.act_id, M=M)
-
-    def _heads(self, a_last, c_last, head, M):
-        """head[:, 0] = value, head[:, 1:] = logits (one GEMM when the trunk is shared)"""
-        m = self.model
-        wh, bh = m.view('W_head'), m.view('b_head')
-        if not m.separate:
-            ops.linear_fwd(a_last, wh, bh, head, 0, M=M)
-            return
-        # separate trunks: two skinny GEMMs into strided halves of the same head buffer is not expressible with linear_fwd's dense
-        # output, so the value and the logits go to their own dense buffers
-        ops.linear_fwd(c_last, wh[:1], bh[:1], self._val_buf(M), 0, M=M)
-        ops.linear_fwd(a_last, wh[1:], bh[1:], self._logit_buf(M), 0, M=M)
-
-    def _val_buf(self, M):
-        if not hasattr(self, '_vb'):
-            self._vb = {}
-        return self._vb.setdefault(M, torch.zeros(M, 1, dtype=torch.float32, device=self.device_t))
-
-    def _logit_buf(self, M):
-        if not hasattr(self, '_lb'):
-            self._lb = {}
-        return self._lb.setdefault(M, torch.zeros(M, self.actions_num, dtype=torch.float32, device=self.device_t))
-
-    def _head_views(self, head, M):
-        """(logits, ld, value, value_ld) of the forward buffers for M rows"""
-        K = self.actions_num
-        if self.model.separate:
-            return self._logit_buf(M), K, self._val_buf(M), 1
-        return head[:, 1:], K + 1, head, K + 1
+        layerwise.forward(self.kernels, m.actor_mlp, x, acts_a, M, m.D, rows_per_chunk, chunk_stride, self.obs_norm)
+        if m.separate:
+            layerwise.forward(self.kernels, m.critic_mlp, x, acts_c, M, m.D, rows_per_chunk, chunk_stride, self.obs_norm)
 
     # =============================================================================== rollout
     def play_steps(self, u=None):
@@ -294,11 +275,8 @@ class DiscreteA2CAgent(A2CBase):
             if self.use_action_masks:          # a2c_common.py:995-997
                 masks = self._to_dev(self.vec_env.get_action_masks()).to(torch.uint8).contiguous()
                 self.action_masks[t].copy_(masks)
-            self._trunk(m.trunk('actor'), obs, self.r_a, N)
-            if m.separate:
-                self._trunk(m.trunk('critic'), obs, self.r_c, N)
-            self._heads(self.r_a[-1], self.r_c[-1], self.r_head, N)
-            lg, ld, vl, vld = self._head_views(self.r_head, N)
+            self._forward(obs, self.r_a, self.r_c, N)
+            lg, ld, vl, vld = self.r_out
             ops.categorical_sample(lg, ld, K, vl, vld, masks, None if u is None else u[t].contiguous(), self.rng_seed, self.rng_epoch, t,
                                    None if vm is None else vm.running_mean, None if vm is None else vm.running_var, self.normalize_value,
                                    self.actions[t], self.neglogpacs[t], self.values[t], self.dones, self.dones_buf[t], self.prev_dones,
@@ -315,11 +293,8 @@ class DiscreteA2CAgent(A2CBase):
             elif getattr(self.algo_observer, 'wants_infos', False):
                 self.algo_observer.process_infos(infos, None)
         # get_values (a2c_common.py:603-626): the reference's forward samples here too; only the value is used
-        self._trunk(m.trunk('actor'), self.obs, self.r_a, N)
-        if m.separate:
-            self._trunk(m.trunk('critic'), self.obs, self.r_c, N)
-        self._heads(self.r_a[-1], self.r_c[-1], self.r_head, N)
-        lg, ld, vl, vld = self._head_views(self.r_head, N)
+        self._forward(self.obs, self.r_a, self.r_c, N)
+        lg, ld, vl, vld = self.r_out
         ops.categorical_sample(None, ld, K, vl, vld, None, None, 0, None, 0, None if vm is None else vm.running_mean,
                                None if vm is None else vm.running_var, self.normalize_value, None, None, self.last_values, None, None,
                                None, None, N, values_only=True)
@@ -356,15 +331,9 @@ class DiscreteA2CAgent(A2CBase):
             r = m.running_mean_std
             ops.moments_update(x, m.D, epm, H, N, r.running_mean, r.running_var, r.count, r.mean_f32, r.std_f32, self.mom_scratch,
                                self.counters[1:2])
-        self._trunk(m.trunk('actor'), x, self.t_a, mb, rows_per_chunk=epm, chunk_stride=N)
-        if m.separate:
-            self._trunk(m.trunk('critic'), x, self.t_c, mb, rows_per_chunk=epm, chunk_stride=N)
-        self._heads(self.t_a[-1], self.t_c[-1], self.t_head, mb)
-        lg, ld, vl, vld = self._head_views(self.t_head, mb)
-        if m.separate:
-            d_lg, d_ld, d_vl, d_vld = self._dl_buf(), K, self._dv_buf(), 1
-        else:
-            d_lg, d_ld, d_vl, d_vld = self.d_head[:, 1:], K + 1, self.d_head, K + 1
+        self._forward(x, self.t_a, self.t_c, mb, rows_per_chunk=epm, chunk_stride=N)
+        lg, ld, vl, vld = self.t_out
+        d_lg, d_ld, d_vl, d_vld = self.d_out
         cfg = ops.CatLossCfg(float(self.e_clip), float(self.critic_coef), float(self.entropy_coef), int(bool(self.clip_value)),
                              int(bool(self.use_smooth_clamp)), int(bool(self.ppo)))
         nb = ops.categorical_loss(lg, ld, K, vl, vld, self.actions[0, e0:], None if self.action_masks is None else self.action_masks[0, e0:],
@@ -375,50 +344,16 @@ class DiscreteA2CAgent(A2CBase):
         stats = self.loss_partials[:nb, :4].sum(dim=0).float()
         if self.diag_on:            # (sum mask, sum mask * clipped) of the minibatch: its clip fraction for diagnostics/clip_frac
             self._diag_clip.append(self.loss_partials[:nb, 4:6].sum(dim=0))
-        # ---- backward through the heads and the trunk(s): split partial gradients, then one reduction ----
-        off_wh, _ = m.layout['W_head']
-        off_bh, _ = m.layout['b_head']
-        nm, ns = self._norm()
+        # ---- backward through the MLP(s): split partial gradients, then one reduction ----
+        layerwise.backward(self.kernels, m.actor_mlp, x, self.t_a, self.d_a, self.part, P, S, mb, m.D, epm, N, self.obs_norm)
         if m.separate:
-            Hl = m.Hl
-            ops.linear_bwd_weight(d_vl, self.t_c[-1], self.part[0, off_wh:], self.part[0, off_bh:], Hl, 1, S, M=mb, split_stride=P)
-            ops.linear_bwd_weight(d_lg, self.t_a[-1], self.part[0, off_wh + Hl:], self.part[0, off_bh + 1:], Hl, K, S, M=mb, split_stride=P)
-            wh = m.view('W_head')
-            ops.linear_bwd_data(d_vl, wh[:1], self.t_c[-1], self.d_c[-1], m.act_id, M=mb)
-            ops.linear_bwd_data(d_lg, wh[1:], self.t_a[-1], self.d_a[-1], m.act_id, M=mb)
-            trunks = [('a', self.t_a, self.d_a), ('c', self.t_c, self.d_c)]
-        else:
-            ops.linear_bwd_weight(self.d_head, self.t_a[-1], self.part[0, off_wh:], self.part[0, off_bh:], m.Hl, 1 + K, S, M=mb,
-                                  split_stride=P)
-            ops.linear_bwd_data(self.d_head, m.view('W_head'), self.t_a[-1], self.d_a[-1], m.act_id, M=mb)
-            trunks = [('a', self.t_a, self.d_a)]
-        for p, acts, dacts in trunks:
-            for l in range(len(m.units) - 1, -1, -1):
-                off_w, shp = m.layout[f'W{p}{l}']
-                off_b, _ = m.layout[f'b{p}{l}']
-                if l > 0:
-                    ops.linear_bwd_weight(dacts[l], acts[l - 1], self.part[0, off_w:], self.part[0, off_b:], shp[1], shp[0], S, M=mb,
-                                          split_stride=P)
-                    ops.linear_bwd_data(dacts[l], m.view(f'W{p}{l}'), acts[l - 1], dacts[l - 1], m.act_id, M=mb)
-                else:
-                    ops.linear_bwd_weight(dacts[0], x, self.part[0, off_w:], self.part[0, off_b:], shp[1], shp[0], S, rows_per_chunk=epm,
-                                          chunk_stride=N, x_ld=m.D, norm_mean=nm, norm_std=ns, M=mb, split_stride=P)
+            layerwise.backward(self.kernels, m.critic_mlp, x, self.t_c, self.d_c, self.part, P, S, mb, m.D, epm, N, self.obs_norm)
         ops.reduce_splits(self.part, self.grad, P, S, split_stride=P)
         if self.multi_gpu:          # a2c_common.py:493-509 (the Adam kernel applies the 1/world scale)
             dist.all_reduce(self.grad, op=dist.ReduceOp.SUM)
         ops.adam_step(m.flat, self.grad, m.exp_avg, m.exp_avg_sq, self.opt_state, None, self.opt_cfg, self.adam_stats, self.counters[2:3],
                       n=P)
         return stats
-
-    def _dl_buf(self):
-        if not hasattr(self, '_dlb'):
-            self._dlb = torch.zeros(self.minibatch_size, self.actions_num, dtype=torch.float32, device=self.device_t)
-        return self._dlb
-
-    def _dv_buf(self):
-        if not hasattr(self, '_dvb'):
-            self._dvb = torch.zeros(self.minibatch_size, 1, dtype=torch.float32, device=self.device_t)
-        return self._dvb
 
     def train_epoch(self, u=None):
         """DiscreteA2CBase.train_epoch (a2c_common.py:1233-1289): returns the reference's tuple."""

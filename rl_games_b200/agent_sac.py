@@ -16,9 +16,9 @@ from datetime import datetime
 import numpy as np
 import torch
 
-from . import ops
+from . import layerwise, ops
 from .common import DefaultAlgoObserver, DefaultRewardsShaper, create_vec_env, make_summary_writer
-from .model import CompileTolerantModel, resolve_device
+from .model import CompileTolerantModel, _RunningStats, resolve_device
 from .model_sac import SACModel
 
 MIN_ALPHA = 0.01        # sac_agent.py base_init: the fixed floor of the actor loss's alpha
@@ -181,16 +181,19 @@ class SACAgent(CompileTolerantModel):
         self.acts_a = [f(B, w) for w in u] + [f(B, 2 * A)]               # actor trunk activations + head
         self.acts_q = [[f(B, w) for w in u] + [f(B, 1)] for _ in range(2)]
         self.acts_t = [[f(B, w) for w in u] + [f(B, 1)] for _ in range(2)]
-        self.d_act = [f(B, w) for w in u]
+        # gradients of the actor and of the two critics: shared hidden-layer scratch, each net's own output gradient
+        d_act = [f(B, w) for w in u]
         self.d_out = [f(B, 1), f(B, 1)]
         self.d_head = f(B, 2 * A)
+        self.grads_q = [d_act + [d] for d in self.d_out]
+        self.grads_a = d_act + [self.d_head]
         self.dx_in = [f(B, D + A), f(B, D + A)]
         self.eps_pi = f(B, A)
         self.logp_next, self.logp_pi = f(B), f(B)
         self.roll_acts = [f(N, w) for w in u] + [f(N, 2 * A)]
         self.actions = f(N, A)
         self.obs_buf = f(N, D)
-        self.n_splits = max(1, min(64, B // 256))
+        self.n_splits = layerwise.n_splits(B)
         m = self.model
         self.part_a = f(self.n_splits, m.actor.n)
         self.part_c = f(self.n_splits, m.critic.n)
@@ -204,10 +207,11 @@ class SACAgent(CompileTolerantModel):
         if self.normalize_input:
             self.rms_scratch = torch.zeros(ops.NUM_SMS * 2 * D, dtype=torch.float64, device=dev)
             self.rms_counter = torch.zeros(1, dtype=torch.int32, device=dev)
-        if self.mixed_precision:
-            self._fwd, self._bwd_data, self._bwd_w = ops.linear_fwd_tc, ops.linear_bwd_data_tc, ops.linear_bwd_weight_tc
-        else:
-            self._fwd, self._bwd_data, self._bwd_w = ops.linear_fwd, ops.linear_bwd_data, ops.linear_bwd_weight
+        self.obs_norm = _RunningStats.f32_pair(self.model.running_mean_std)
+        # the passes the reference runs outside autocast -- the critic target's actor and target critics (sac_agent.py update_critic),
+        # the rollout's act() -- run on the fp32 kernels whatever mixed_precision says
+        self.k32 = layerwise.Kernels()
+        self.kernels = layerwise.Kernels(tc=self.mixed_precision)
 
     def init_tensors(self):
         self.ep_state.zero_()
@@ -216,34 +220,6 @@ class SACAgent(CompileTolerantModel):
     @property
     def alpha(self):
         return self.model.log_alpha.exp()
-
-    # =============================================================================== MLP passes
-    def _mlp_fwd(self, layers, x, x_ld, K0, acts, M, norm=None, fp32=False):
-        """fp32=True: the fp32 kernels whatever mixed_precision says -- the passes the reference runs outside autocast (the critic target's
-        actor and target critics, sac_agent.py update_critic; the rollout's act())"""
-        L = len(layers)
-        fwd = ops.linear_fwd if fp32 else self._fwd
-        for l, (W, b) in enumerate(layers):
-            X, ld, K = (x, x_ld, K0) if l == 0 else (acts[l - 1], W.shape[1], W.shape[1])
-            nm, ns = norm if (l == 0 and norm is not None) else (None, None)
-            fwd(X, W, b, acts[l], self.model.act_id if l < L - 1 else 0, x_ld=ld, norm_mean=nm, norm_std=ns, M=M)
-
-    def _mlp_bwd(self, arena, prefix, layers, x, x_ld, acts, d_top, part, M, dx_out=None, weights=True):
-        """gradients of one MLP into `part` (split partials of `arena`) and, with dx_out, dL/d(input) into dx_out"""
-        L, act = len(layers), self.model.act_id
-        pre = 'trunk.' if prefix == '' else prefix
-        dY = d_top
-        for l in range(L - 1, -1, -1):
-            W, _ = layers[l]
-            X, ld = (x, x_ld) if l == 0 else (acts[l - 1], W.shape[1])
-            if weights:
-                ow, ob = arena.layout[f'{pre}{2 * l}.weight'][0], arena.layout[f'{pre}{2 * l}.bias'][0]
-                self._bwd_w(dY, X, part[0, ow:], part[0, ob:], W.shape[1], W.shape[0], self.n_splits, x_ld=ld, M=M, split_stride=arena.n)
-            if l > 0:
-                self._bwd_data(dY, W, acts[l - 1], self.d_act[l - 1], act, M=M)
-                dY = self.d_act[l - 1]
-            elif dx_out is not None:
-                self._bwd_data(dY, W, None, dx_out, 0, M=M)
 
     def _adam(self, i, params, grads, m, v, n):
         ops.adam_step(params, grads, m, v, self.opt_state[i], None, self.opt_cfg[i], None, self.counters[i:i + 1], n=n)
@@ -269,39 +245,39 @@ class SACAgent(CompileTolerantModel):
     def _update(self, stats_row, actor_step):
         m, B, D, A = self.model, self.batch_size, self.D, self.A
         ld = D + A
-        norm = (m.running_mean_std.mean_f32, m.running_mean_std.std_f32) if self.normalize_input else (None, None)
-        ops.sac_replay_sample(self.rb, B, self._tb_get('idx'), self.seed, self.rng_ctr, norm[0], norm[1], self.x_cur, self.x_pi, self.x_next,
+        fwd, bwd, k = layerwise.forward, layerwise.backward, self.kernels
+        nm, ns = self.obs_norm
+        ops.sac_replay_sample(self.rb, B, self._tb_get('idx'), self.seed, self.rng_ctr, nm, ns, self.x_cur, self.x_pi, self.x_next,
                               self.reward_b, self.not_done_b)
         # ---- update_critic: target from the next observations (actor + target critics, no gradients)
-        actor_l = m.layers(m.actor)
-        self._mlp_fwd(actor_l, self.x_next, ld, D, self.acts_a, B, fp32=True)
+        fwd(self.k32, m.actor_mlp, self.x_next, self.acts_a, B, ld)
         ops.sac_squash_fwd(self.acts_a[-1], B, A, m.log_std_bounds, self._tb_get('noise_next'), self.seed, self.rng_ctr, ops.SAC_SITE_NEXT,
                            self.act_box, self.log_action_scale_sum, dst=self.x_next[:, D:], dst_ld=ld, logp=self.logp_next)
-        for k, q in enumerate(('Q1.', 'Q2.')):
-            self._mlp_fwd(m.layers(m.critic_target, q), self.x_next, ld, ld, self.acts_t[k], B, fp32=True)
-            self._mlp_fwd(m.layers(m.critic, q), self.x_cur, ld, ld, self.acts_q[k], B)
+        for q in range(2):
+            fwd(self.k32, m.target_mlps[q], self.x_next, self.acts_t[q], B, ld)
+            fwd(k, m.critic_mlps[q], self.x_cur, self.acts_q[q], B, ld)
         ops.sac_critic_loss(self.acts_q[0][-1], self.acts_q[1][-1], self.acts_t[0][-1], self.acts_t[1][-1], self.logp_next, self.reward_b,
                             self.not_done_b, m.log_alpha, self.gamma, B, self.d_out[0], self.d_out[1], stats_row)
-        for k, q in enumerate(('Q1.', 'Q2.')):
-            self._mlp_bwd(m.critic, q, m.layers(m.critic, q), self.x_cur, ld, self.acts_q[k], self.d_out[k], self.part_c, B)
+        for q in range(2):
+            bwd(k, m.critic_mlps[q], self.x_cur, self.acts_q[q], self.grads_q[q], self.part_c, m.critic.n, self.n_splits, B, ld)
         ops.reduce_splits(self.part_c, m.critic.grad, m.critic.n, self.n_splits)
         self._adam(1, m.critic.flat, m.critic.grad, m.critic.exp_avg, m.critic.exp_avg_sq, m.critic.n)
         # ---- update_actor_and_alpha (every policy_frequency-th update), on the updated critic
         if actor_step:
-            self._mlp_fwd(actor_l, self.x_pi, ld, D, self.acts_a, B)
+            fwd(k, m.actor_mlp, self.x_pi, self.acts_a, B, ld)
             ops.sac_squash_fwd(self.acts_a[-1], B, A, m.log_std_bounds, self._tb_get('noise_actor'), self.seed, self.rng_ctr, ops.SAC_SITE_ACTOR,
                                self.act_box, self.log_action_scale_sum, dst=self.x_pi[:, D:], dst_ld=ld, eps_out=self.eps_pi,
                                logp=self.logp_pi)
-            for k, q in enumerate(('Q1.', 'Q2.')):
-                self._mlp_fwd(m.layers(m.critic, q), self.x_pi, ld, ld, self.acts_q[k], B)
+            for q in range(2):
+                fwd(k, m.critic_mlps[q], self.x_pi, self.acts_q[q], B, ld)
             ops.sac_actor_loss(self.acts_q[0][-1], self.acts_q[1][-1], self.logp_pi, m.log_alpha, MIN_ALPHA, self.target_entropy,
                                self.learnable_temperature, B, self.d_out[0], self.d_out[1], m.log_alpha_grad, stats_row)
-            for k, q in enumerate(('Q1.', 'Q2.')):       # critic weights get no update from this pass: input gradients only
-                self._mlp_bwd(m.critic, q, m.layers(m.critic, q), self.x_pi, ld, self.acts_q[k], self.d_out[k], None, B,
-                              dx_out=self.dx_in[k], weights=False)
+            for q in range(2):       # critic weights get no update from this pass: input gradients only
+                bwd(k, m.critic_mlps[q], self.x_pi, self.acts_q[q], self.grads_q[q], None, m.critic.n, self.n_splits, B, ld,
+                    dx_out=self.dx_in[q], weights=False)
             ops.sac_squash_bwd(self.acts_a[-1], self.eps_pi, B, A, m.log_std_bounds, self.act_box, self.dx_in[0][:, D:], self.dx_in[1][:, D:],
                                ld, m.log_alpha, MIN_ALPHA, self.d_head)
-            self._mlp_bwd(m.actor, '', actor_l, self.x_pi, ld, self.acts_a, self.d_head, self.part_a, B)
+            bwd(k, m.actor_mlp, self.x_pi, self.acts_a, self.grads_a, self.part_a, m.actor.n, self.n_splits, B, ld)
             ops.reduce_splits(self.part_a, m.actor.grad, m.actor.n, self.n_splits)
             self._adam(0, m.actor.flat, m.actor.grad, m.actor.exp_avg, m.actor.exp_avg_sq, m.actor.n)
             if self.learnable_temperature:
@@ -370,8 +346,7 @@ class SACAgent(CompileTolerantModel):
         if random_exploration:
             ops.sac_uniform_actions(self.action_low, self.action_high, self._tape('u'), self.seed, self.roll_ctr, self.actions, N, self.A)
         else:
-            norm = (m.running_mean_std.mean_f32, m.running_mean_std.std_f32) if self.normalize_input else None
-            self._mlp_fwd(m.layers(m.actor), obs, self.D, self.D, self.roll_acts, N, norm=norm, fp32=True)
+            layerwise.forward(self.k32, m.actor_mlp, obs, self.roll_acts, N, self.D, norm=self.obs_norm)
             ops.sac_squash_fwd(self.roll_acts[-1], N, self.A, m.log_std_bounds, self._tape('noise_roll'), self.seed, self.roll_ctr,
                                ops.SAC_SITE_ROLLOUT, self.act_box, 0.0, dst=self.actions, dst_ld=self.A)
         ops.bump_u64(self.roll_ctr)

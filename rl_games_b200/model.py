@@ -30,6 +30,7 @@ from collections import OrderedDict
 import torch
 
 from . import ops
+from .layerwise import Layer
 
 
 def _apply_init(t, spec, fan_in):
@@ -82,6 +83,11 @@ class _RunningStats:
 
     def refresh(self):
         ops.refresh_norm(self.running_mean, self.running_var, self.mean_f32, self.std_f32)
+
+    @staticmethod
+    def f32_pair(stats):
+        """(mean_f32, std_f32) of `stats`, the `norm` operands of the kernels; (None, None) without a normaliser"""
+        return (None, None) if stats is None else (stats.mean_f32, stats.std_f32)
 
     def state_dict(self, prefix):
         return OrderedDict([(prefix + 'running_mean', self.running_mean.clone()),
@@ -344,6 +350,7 @@ class B200Model(FlatParamModel):
         self.grad = torch.zeros(off, dtype=torch.float32, device=self.device)
         self.W = [self.view(f'W{i}') for i in range(len(self.units))]
         self.b = [self.view(f'b{i}') for i in range(len(self.units))]
+        self.mlp = [Layer(self.W[i], self.b[i], self.layout[f'W{i}'][0], self.layout[f'b{i}'][0], self.act_id) for i in range(len(self.units))]
         self.sigma = self.view('sigma')
         if self.sigma_transform:
             # what the kernels are handed instead of the raw parameter, and the chain factor of its gradient (refresh_sigma_floor)
@@ -360,10 +367,7 @@ class B200Model(FlatParamModel):
             self.grad_mask = torch.zeros(off, dtype=torch.float32, device=self.device)
             for v in self._param_views(self.grad_mask):
                 v.fill_(1.0)
-        self.gW = [self.view(f'W{i}', self.grad) for i in range(len(self.units))]
-        self.gb = [self.view(f'b{i}', self.grad) for i in range(len(self.units))]
         self.g_sigma = self.view('sigma', self.grad)
-        self.gW_head, self.gb_head = self.view('W_head', self.grad), self.view('b_head', self.grad)
         self.running_mean_std = _RunningStats(self.D, self.device) if self.normalize_input else None
         self.value_mean_std = _RunningStats(1, self.device)   # always allocated; used iff normalize_value
         self.a2c_network = _NetworkView(self)

@@ -17,6 +17,7 @@ from collections import OrderedDict
 import torch
 
 from . import ops
+from .layerwise import Layer
 from .model import _RunningStats, _apply_init, _model_call
 
 
@@ -97,6 +98,9 @@ class SACModel:
         self.log_alpha_v = torch.zeros(1, dtype=torch.float32, device=device)
         self.running_mean_std = _RunningStats(obs_dim, device) if self.normalize_input else None
         self._init_weights()
+        self.actor_mlp = self.layers(self.actor)
+        self.critic_mlps = [self.layers(self.critic, q) for q in ('Q1.', 'Q2.')]
+        self.target_mlps = [self.layers(self.critic_target, q) for q in ('Q1.', 'Q2.')]
 
     # ------------------------------------------------------------------------------------------------ init (SACBuilder.Network)
     def _init_weights(self):
@@ -128,9 +132,13 @@ class SACModel:
 
     # ------------------------------------------------------------------------------------------------ layer views
     def layers(self, arena, prefix=''):
-        """[(W, b)] of one MLP: prefix '' = the actor trunk, 'Q1.' / 'Q2.' = a critic"""
+        """layer records of one MLP (linear output layer): prefix '' = the actor trunk + head, 'Q1.' / 'Q2.' = a critic"""
         pre = 'trunk.' if prefix == '' else prefix
-        return [(arena.view(f'{pre}{2 * i}.weight'), arena.view(f'{pre}{2 * i}.bias')) for i in range(self.n_layers)]
+        out = []
+        for i in range(self.n_layers):
+            w, b = f'{pre}{2 * i}.weight', f'{pre}{2 * i}.bias'
+            out.append(Layer(arena.view(w), arena.view(b), arena.layout[w][0], arena.layout[b][0], self.act_id if i < self.n_layers - 1 else 0))
+        return out
 
     # ------------------------------------------------------------------------------------------------ state dicts
     def part_state_dict(self, part):

@@ -330,9 +330,13 @@ def test_mixed_precision_auto_resolves_by_geometry_and_explicit_true_never_downg
     c = _build(monkeypatch, tmp_path, g, _Env(g), tc=False, over={'mixed_precision': True})
     assert c.mixed_precision is True and c.use_tc is False and c.gemm_tc is True
     from rl_games_b200 import ops
-    assert c._lin_bww is ops.linear_bwd_weight_tc and c._lin_fwd is not ops.linear_fwd
     c.init_tensors()
-    assert c._lin_fwd.func is ops.linear_fwd_tc and c._lin_bwd.func is ops.linear_bwd_data_tc and c.wbf.dtype == torch.bfloat16
+    k = c.kernels
+    assert k.bwd_weight is ops.linear_bwd_weight_tc and k.fwd.func is ops.linear_fwd_tc and k.bwd_data.func is ops.linear_bwd_data_tc
+    # forward and data gradient read their weight operands from the bf16 twin of the parameter arena
+    for f in (k.fwd, k.bwd_data):
+        assert f.keywords['bf16_arena'][0] is c.model.flat and f.keywords['bf16_arena'][1] is c.wbf
+    assert c.wbf.dtype == torch.bfloat16
     g2 = dict(torch.load(os.path.join(GOLDEN, 'agent_tcshape.pt'), weights_only=False))
     import _torch_ops
     _torch_ops.install_tc(monkeypatch)          # its tc_supported stand-in accepts the fixture's small three-layer geometry
