@@ -129,6 +129,12 @@ int b200rl_moments_update_f64(const float* x, int D, int rows_per_chunk, int n_c
  *  scratch: double[scratch_blocks*2*D].  Requires D % 4 == 0 (else use b200rl_moments_update_f64 per minibatch). */
 int b200rl_obs_mb_moments_f64(const float* x, int D, int H, int N, int envs_per_mb, const double* run_mean,
                               double* mbmom, float* mb_shift, double* scratch, int scratch_blocks, int* counters, void* stream);
+/* moments_update on uint8 rows (image observations): the batch moments of x * 1/255 (a2c_common.py:972-983), merged as
+ * b200rl_moments_update_f64 merges them.  Needs no scratch: one CTA owns 32 columns over all rows (deterministic).  Two launches: the
+ * columns, then the count. */
+int b200rl_moments_update_u8_f64(const uint8_t* x, int D, int rows_per_chunk, int n_chunks, int64_t chunk_stride,
+                                 double* mean, double* var, int64_t* count, float* mean_f32, float* std_f32, float eps,
+                                 void* stream);
 int b200rl_obs_stats_merge_f64(const double* mbmom_i, const float* mb_shift, int D, int n_rows, double* mean, double* var,
                                int64_t* count, float* mean_f32, float* std_f32, float eps, void* stream);
 /* mean_f32 = (float)mean, std_f32 = sqrt((float)var + eps): the fp32 copies the fused kernels consume */
@@ -154,6 +160,26 @@ int b200rl_linear_bwd_data_f32(const float* dY, const float* W, const float* A_p
 int b200rl_linear_bwd_weight_f32(const float* dY, const float* X, int rows_per_chunk, int64_t chunk_stride,
                                  int64_t x_ld, const float* norm_mean, const float* norm_std,
                                  float* dW_part, float* db_part, int64_t split_stride, int M, int K, int Nout,
+                                 int n_splits, void* stream);
+/* ---------------------------------------------------------------------------------------------
+ * fp32 2-D convolutions of an image trunk (network_builder.py:161-181, plain conv2d), implicit GEMM on the CUDA cores.
+ * Geometry: input [C, H, W], Cout filters W[Cout, C, KH, KW] (PyTorch's layout), one stride and one zero padding for both axes,
+ * output [Cout, Ho, Wo], Ho = (H + 2 pad - KH) / stride + 1.  Activations and gradients are dense NCHW rows of M samples.
+ *   conv2d_fwd:        Y = act(conv(norm(X)) + b); X rows chunked like linear_fwd's (arena rows), uint8 (x_u8: scaled by 1/255)
+ *                      or fp32, NHWC (x_nhwc: the env's [H, W, C] frames, permute_input) or NCHW; the optional normaliser
+ *                      (norm_mean / norm_std, C*H*W each) indexes the env's own layout and is applied before zero padding.
+ *   conv2d_bwd_data:   dX = conv^T(dY, W) * act'(A_prev), gathered per input pixel (deterministic, no atomics).
+ *   conv2d_bwd_weight: dW_part[s*split_stride + ..][Cout, C*KH*KW] = sum over the output pixels of row split s, db_part likewise;
+ *                      X read as conv2d_fwd reads it.
+ * ------------------------------------------------------------------------------------------- */
+int b200rl_conv2d_fwd_f32(const void* X, int x_u8, int x_nhwc, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
+                          const float* norm_mean, const float* norm_std, const float* W, const float* b, float* Y,
+                          int M, int C, int H, int Wd, int Cout, int KH, int KW, int stride, int pad, int act, void* stream);
+int b200rl_conv2d_bwd_data_f32(const float* dY, const float* W, const float* A_prev, float* dX, int M, int C, int H, int Wd,
+                               int Cout, int KH, int KW, int stride, int pad, int act_prev, void* stream);
+int b200rl_conv2d_bwd_weight_f32(const float* dY, const void* X, int x_u8, int x_nhwc, int rows_per_chunk, int64_t chunk_stride,
+                                 int64_t x_ld, const float* norm_mean, const float* norm_std, float* dW_part, float* db_part,
+                                 int64_t split_stride, int M, int C, int H, int Wd, int Cout, int KH, int KW, int stride, int pad,
                                  int n_splits, void* stream);
 /* out[i] = sum_s part[s*split_stride + i]  (deterministic, fixed order) */
 /* The same three building blocks on the tensor cores (wgmma, bf16 operands rounded while they are staged, fp32 accumulate in

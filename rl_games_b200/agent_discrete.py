@@ -7,7 +7,8 @@ STATUS: parity-green on an H100 (``tests/test_discrete_gpu.py``) against a CPU o
 (csrc/discrete.cu) reuses the kernels of the continuous path: linear_fwd / linear_bwd_* / reduce_splits (mlp_simt.cu), gae_fused, prepare_batch, moments_update,
 mask_inv_counts (stats.cu, gae.cu), post_step (rollout.cu), adam_step (adam.cu).
 
-Scope of this first edition: one GPU, eager launches (no CUDA graph), flat Box observations, ``Discrete(K)`` or multi-discrete
+Image observations (``cnn: {type: conv2d}`` on a rank-3 Box) run a conv trunk (csrc/conv.cu) in front of the MLP; see DESIGN.md §4.
+Scope of this first edition: one GPU, eager launches (no CUDA graph), flat Box observations or conv2d frames, ``Discrete(K)`` or multi-discrete
 ``Tuple(Discrete(K_j))`` action spaces (K_j <= 64, <= 8 heads), no RNN, no central value.  The scheduler steps once per MINI-EPOCH on the mean KL like the reference
 (a2c_common.py:1265-1272), which costs one host sync per mini-epoch.
 
@@ -24,13 +25,17 @@ from . import layerwise, ops
 from .a2c_base import A2CBase
 from .common import make_summary_writer
 from .layerwise import Layer
-from .model import check_network_params, FlatParamModel, _RunningStats
+from .model import _apply_init, check_network_params, FlatParamModel, _RunningStats
 
 
 class DiscreteModel(FlatParamModel):
-    """Flat fp32 parameter arena of A2CBuilder.Network for a discrete space.  Arena order: actor trunk, [critic trunk], fused head
-    W_head [1 + K, Hl] (row 0 = value, rows 1.. = logits) and b_head [1 + K]; ``_param_views`` lists the tensors in the reference's
-    ``model.parameters()`` order (actor_mlp.*, critic_mlp.*, value.*, logits.*) for state dicts and the index-keyed Adam state."""
+    """Flat fp32 parameter arena of A2CBuilder.Network for a discrete space.  Arena order: [actor conv trunk, [critic conv trunk]],
+    actor MLP, [critic MLP], fused head W_head [1 + K, Hl] (row 0 = value, rows 1.. = logits) and b_head [1 + K]; ``_param_views``
+    lists the tensors in the reference's ``model.parameters()`` order (actor_cnn.*, critic_cnn.*, actor_mlp.*, critic_mlp.*, value.*,
+    logits.*) for state dicts and the index-keyed Adam state.
+
+    ``obs_dim`` is the flat observation size, or the observation shape: a rank-3 shape with a plain ``conv2d`` cnn
+    (network_builder.py:161-181) puts a convolutional trunk in front of each MLP."""
 
     def __init__(self, network_params, obs_dim, n_actions, device, normalize_input, normalize_value, head_sizes=None):
         self.head_sizes = list(head_sizes) if head_sizes else None          # multi-discrete: one logits head per Tuple component
@@ -43,28 +48,38 @@ class DiscreteModel(FlatParamModel):
         if self.activation not in ops.ACT:
             raise NotImplementedError(f'activation {self.activation}')
         self.act_id = ops.ACT[self.activation]
-        if mlp.get('initializer', {'name': 'default'}).get('name', 'default') != 'default':
+        if 'rnn' in network_params:
+            raise NotImplementedError("'rnn' networks are not supported by the discrete B200 agent yet")
+        self.obs_shape = tuple(obs_dim) if isinstance(obs_dim, (tuple, list, torch.Size)) else (int(obs_dim),)
+        self.cnn = _ConvTrunk(network_params['cnn'], self.obs_shape) if 'cnn' in network_params else None
+        mlp_init = mlp.get('initializer', {'name': 'default'})
+        if self.cnn is None and mlp_init.get('name', 'default') != 'default':
             raise NotImplementedError("only the 'default' mlp initializer is mirrored for discrete models")
-        for k in ('cnn', 'rnn'):
-            if k in network_params:
-                raise NotImplementedError(f"'{k}' networks are not supported by the discrete B200 agent yet")
         self.separate = bool(network_params.get('separate', False))
-        self.D, self.K = int(obs_dim), int(n_actions)
+        self.D, self.K = int(np.prod(self.obs_shape)), int(n_actions)
+        self.mlp_in = self.cnn.out_size if self.cnn else self.D
         self.device = torch.device(device)
         self.normalize_input, self.normalize_value = bool(normalize_input), bool(normalize_value)
-        sizes, ins = [], self.D
+        sizes = []
+        for p in (['a', 'c'] if self.separate and self.cnn else ['a'] if self.cnn else []):
+            for i, (shp, _) in enumerate(self.cnn.layers):
+                sizes += [(f'K{p}{i}', shp), (f'k{p}{i}', (shp[0],))]
+        ins = self.mlp_in
         for i, u in enumerate(self.units):
             sizes += [(f'Wa{i}', (u, ins)), (f'ba{i}', (u,))]
             ins = u
         if self.separate:
-            ins = self.D
+            ins = self.mlp_in
             for i, u in enumerate(self.units):
                 sizes += [(f'Wc{i}', (u, ins)), (f'bc{i}', (u,))]
                 ins = u
         self.Hl = ins
         sizes += [('W_head', (1 + self.K, ins)), ('b_head', (1 + self.K,))]
         self._init_arena(sizes)
-        self._init_linear_default()          # network_builder.py:332-340 with the 'default' initializer
+        if self.cnn:
+            self._init_like_reference(mlp_init)
+        else:
+            self._init_linear_default()          # network_builder.py:332-340 with the 'default' initializer
         self.running_mean_std = _RunningStats(self.D, self.device) if self.normalize_input else None
         self.value_mean_std = _RunningStats(1, self.device) if self.normalize_value else None
         # the head is the linear output layer of the trunk's MLP: one MLP into [value | logits] when the trunk is shared; with separate
@@ -78,6 +93,40 @@ class DiscreteModel(FlatParamModel):
         else:
             self.actor_mlp.append(Layer(wh, bh, off_wh, off_bh, 0))
             self.critic_mlp = None
+        # conv trunks: layer records of the actor's (shared) trunk and of the critic's; the conv parameters lead the arena
+        self.actor_conv = self._conv_layers('a') if self.cnn else None
+        self.critic_conv = self._conv_layers('c') if self.cnn and self.separate else None
+        self.conv_params = self.layout['Wa0'][0]
+
+    def _conv_layers(self, p):
+        return [Layer(self.view(f'K{p}{i}'), self.view(f'k{p}{i}'), self.layout[f'K{p}{i}'][0], self.layout[f'k{p}{i}'][0], self.cnn.act)
+                for i in range(len(self.cnn.layers))]
+
+    def _init_like_reference(self, mlp_init):
+        """A2CBuilder.Network.__init__ (network_builder.py:226-341) on torch's global generator, draw for draw: each Conv2d and Linear
+        is constructed (torch's own init) in registration order, _calc_input_size draws its probe frame between the conv trunks and
+        the MLPs, then the init loop applies the cnn initializer to every conv weight and the mlp initializer to every linear weight
+        (a no-op for 'default'), zeroing every bias."""
+        nn = torch.nn
+        convs = [nn.Conv2d(shp[1], shp[0], (shp[2], shp[3]), stride=g[3], padding=g[4]) for _ in range(2 if self.separate else 1)
+                 for shp, g in self.cnn.layers]
+        torch.rand(1, *self.cnn.in_shape)
+        lins, n_trunks = [], 2 if self.separate else 1
+        for _ in range(n_trunks):
+            ins = self.mlp_in
+            for u in self.units:
+                lins.append(nn.Linear(ins, u))
+                ins = u
+        lins.append(nn.Linear(self.Hl, 1))
+        lins += [nn.Linear(self.Hl, k) for k in (self.head_sizes or [self.K])]
+        with torch.no_grad():
+            for mods, spec in ((convs, self.cnn.initializer), (lins, mlp_init)):
+                for mod in mods:
+                    if spec.get('name', 'default') != 'default':
+                        _apply_init(mod.weight, spec, None)
+                    mod.bias.zero_()
+            for v, t in zip(self._param_views(), [t for mod in convs + lins for t in (mod.weight, mod.bias)]):
+                v.copy_(t.reshape(v.shape))
 
     def _trunk_layers(self, p):
         return [Layer(self.view(f'W{p}{i}'), self.view(f'b{p}{i}'), self.layout[f'W{p}{i}'][0], self.layout[f'b{p}{i}'][0], self.act_id)
@@ -85,6 +134,9 @@ class DiscreteModel(FlatParamModel):
 
     def _param_views(self, arena=None):
         out = []
+        for p in (['a', 'c'] if self.separate and self.cnn else ['a'] if self.cnn else []):
+            for i in range(len(self.cnn.layers)):
+                out += [self.view(f'K{p}{i}', arena), self.view(f'k{p}{i}', arena)]
         for p in (['a', 'c'] if self.separate else ['a']):
             for i in range(len(self.units)):
                 out += [self.view(f'W{p}{i}', arena), self.view(f'b{p}{i}', arena)]
@@ -100,6 +152,9 @@ class DiscreteModel(FlatParamModel):
 
     def param_names(self):
         names = []
+        for pre in (['actor_cnn', 'critic_cnn'] if self.separate and self.cnn else ['actor_cnn'] if self.cnn else []):
+            for i in range(len(self.cnn.layers)):
+                names += [f'a2c_network.{pre}.{2 * i}.weight', f'a2c_network.{pre}.{2 * i}.bias']
         for pre in (['actor_mlp', 'critic_mlp'] if self.separate else ['actor_mlp']):
             for i in range(len(self.units)):
                 names += [f'a2c_network.{pre}.{2 * i}.weight', f'a2c_network.{pre}.{2 * i}.bias']
@@ -110,6 +165,51 @@ class DiscreteModel(FlatParamModel):
             names += [f'a2c_network.logits.{j}.weight', f'a2c_network.logits.{j}.bias']
         return names
 
+    def state_dict(self):
+        sd = super().state_dict()
+        if self.cnn and self.normalize_input:        # RunningMeanStd(obs_shape) keeps the frame's shape (models.py:31)
+            for k in ('running_mean_std.running_mean', 'running_mean_std.running_var'):
+                sd[k] = sd[k].reshape(self.obs_shape)
+        return sd
+
+
+class _ConvTrunk:
+    """The geometry of a plain ``conv2d`` cnn (network_builder.py:161-181) on a rank-3 observation.  ``in_shape``: the network's
+    (C, H, W) input, the env's (H, W, C) frame transposed when ``permute_input`` (the default, network_builder.py:360-361);
+    ``layers``: ((Cout, C, KH, KW), (C, H, W, stride, pad)) per conv; ``out_shape`` / ``out_size``: the last conv's output and its
+    flattened size, the MLP's input (_calc_input_size)."""
+
+    REFUSED = {'conv2d_spatial_softargmax': 'a spatial soft-argmax head', 'conv2d_flatten': 'a flatten layer',
+               'coord_conv2d': 'coordinate channels'}
+
+    def __init__(self, cnn, obs_shape):
+        ctype = cnn.get('type')
+        if ctype != 'conv2d':
+            why = self.REFUSED.get(ctype, 'only plain conv2d is built')
+            raise NotImplementedError(f"'cnn' networks of type {ctype!r} ({why}) are not supported by the discrete B200 agent yet")
+        if len(obs_shape) != 3:
+            raise NotImplementedError(f"a 'conv2d' cnn needs a rank-3 Box observation, got shape {tuple(obs_shape)}")
+        self.nhwc = bool(cnn.get('permute_input', True))
+        self.in_shape = (obs_shape[2], obs_shape[0], obs_shape[1]) if self.nhwc else tuple(obs_shape)
+        act = cnn.get('activation', 'relu')
+        if act not in ops.ACT:
+            raise NotImplementedError(f'cnn activation {act}')
+        self.act = ops.ACT[act]
+        self.initializer = dict(cnn.get('initializer') or {'name': 'default'})
+        self.layers = []
+        C, H, W = self.in_shape
+        for conv in cnn['convs']:
+            k, st, pad = conv['kernel_size'], conv['strides'], conv.get('padding', 0)
+            if not all(isinstance(v, int) and not isinstance(v, bool) for v in (k, st, pad)) or k < 1 or st < 1 or pad < 0:
+                raise NotImplementedError(f'conv2d kernel_size / strides / padding must be integers, got {k!r} / {st!r} / {pad!r}')
+            Ho, Wo = (H + 2 * pad - k) // st + 1, (W + 2 * pad - k) // st + 1
+            if Ho < 1 or Wo < 1:
+                raise ValueError(f'conv2d kernel {k} does not fit a {H}x{W} input with padding {pad}')
+            self.layers.append(((int(conv['filters']), C, k, k), (C, H, W, st, pad)))
+            C, H, W = int(conv['filters']), Ho, Wo
+        self.out_shape = (C, H, W)
+        self.out_size = C * H * W
+
 
 class DiscreteA2CAgent(A2CBase):
     # torch_ext.AverageMeter means (float32) for the reward / episode-length summaries
@@ -119,7 +219,7 @@ class DiscreteA2CAgent(A2CBase):
     # Adam kernel (which applies 1/world), the scheduler sees the rank-mean KL
     def __init__(self, base_name, params):
         super().__init__(base_name, params)
-        self.model = DiscreteModel(self.network_params, self.obs_shape[0], self.actions_num, self.device_t, self.normalize_input,
+        self.model = DiscreteModel(self.network_params, self.obs_shape, self.actions_num, self.device_t, self.normalize_input,
                                    self.normalize_value, head_sizes=self.head_sizes)
         self.value_mean_std = self.model.value_mean_std
         self.rng_seed = int(self.config.get('b200_rng_seed', params.get('seed', 0) or 0))
@@ -150,9 +250,13 @@ class DiscreteA2CAgent(A2CBase):
             raise ValueError("PPO next_step autoreset masking does not support multi-agent envs; "
                              "wrap the env with a same_step autoreset adapter instead")
         self.observation_space = self.env_info['observation_space']
-        if type(self.observation_space).__name__ == 'Dict' or len(self.observation_space.shape) != 1:
+        # flat Box observations, or rank-3 frames in front of a cnn (the model checks the cnn); the arena keeps the env's dtype
+        # (experience.py:376): uint8 frames stay bytes and are scaled by 1/255 where the first conv and the normaliser read them
+        is_dict = type(self.observation_space).__name__ == 'Dict'
+        if is_dict or len(self.observation_space.shape) != 1 and ('cnn' not in self.network_params or len(self.observation_space.shape) != 3):
             raise NotImplementedError('only flat Box observations')
         self.obs_shape = self.observation_space.shape
+        self.obs_dtype = torch.uint8 if len(self.obs_shape) == 3 and np.dtype(self.observation_space.dtype) == np.uint8 else torch.float32
         action_space = self.env_info['action_space']
         kind = type(action_space).__name__          # a2c_common.py:1211-1224
         if kind == 'Discrete':
@@ -185,10 +289,11 @@ class DiscreteA2CAgent(A2CBase):
     def init_tensors(self):
         if self._tensors_ready:
             return
-        H, N, D, K, m, mb = self.horizon_length, self.num_rows, self.obs_shape[0], self.actions_num, self.model, self.minibatch_size
+        H, N, K, m, mb = self.horizon_length, self.num_rows, self.actions_num, self.model, self.minibatch_size
+        D = m.D
         dev = self.device_t
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)   # noqa: E731
-        self.obses = f(H, N, D)
+        self.obses = torch.zeros(H, N, D, dtype=self.obs_dtype, device=dev)
         self.actions = (torch.zeros(H, N, len(self.head_sizes), dtype=torch.int64, device=dev) if self.head_sizes
                         else torch.zeros(H, N, dtype=torch.int64, device=dev))
         self.neglogpacs, self.values, self.rewards = f(H, N), f(H, N), f(H, N)
@@ -215,14 +320,26 @@ class DiscreteA2CAgent(A2CBase):
             self.r_c = self.t_c = self.d_c = None
             self.r_out, self.t_out, self.d_out = ((a[-1][:, 1:], K + 1, a[-1], K + 1) for a in (self.r_a, self.t_a, self.d_a))
         self.n_splits = layerwise.n_splits(mb)
-        self.part = f(self.n_splits, m.num_params)
+        if m.cnn:
+            # conv activations (NCHW rows) of each trunk, rollout / training, and their gradients (pre-activation); the conv weight
+            # gradients split over the output pixels' rows, so they take more split rows than the MLP (the leading conv_params columns)
+            conv_bufs = lambda M: [f(M, shp[0], *self._conv_out(g, shp)) for shp, g in m.cnn.layers]   # noqa: E731
+            self.r_ka, self.t_ka, self.d_ka = conv_bufs(N), conv_bufs(mb), conv_bufs(mb)
+            self.r_kc, self.t_kc, self.d_kc = (conv_bufs(N), conv_bufs(mb), conv_bufs(mb)) if m.separate else (None, None, None)
+            self.conv_splits = layerwise.n_splits(mb * m.cnn.out_shape[1] * m.cnn.out_shape[2])
+        else:
+            self.r_ka = self.t_ka = self.d_ka = self.r_kc = self.t_kc = self.d_kc = None
+            self.conv_splits = 0
+        self.part = f(max(self.n_splits, self.conv_splits), m.num_params)
         self.grad = f(m.num_params)
         self.diag_exp_var = f(self.num_minibatches) if self.diag_on else None
         self._diag_clip = []
         self.loss_partials = torch.zeros((mb + 255) // 256, 8, dtype=torch.float64, device=dev)
         self.gae_partials = torch.zeros(max(64, (N + 63) // 64), 8, dtype=torch.float64, device=dev)
         self.inv_counts = f(self.num_minibatches) if self.mask_autoreset_rows else None
-        self.mom_scratch = torch.zeros(ops.NUM_SMS * 4 * 2 * D, dtype=torch.float64, device=dev)
+        # uint8 frames update their statistics without partials (moments_update_u8); fp32 rows need NUM_SMS * 4 partial rows
+        self.mom_scratch = (None if self.obs_dtype == torch.uint8 else
+                            torch.zeros(ops.NUM_SMS * 4 * 2 * D, dtype=torch.float64, device=dev))
         self.post_scratch = torch.zeros(((N + 255) // 256) * 4, dtype=torch.float64, device=dev)
         self.post_ma = ops.post_step_ma_buffers(N, self.num_agents, dev) if self.num_agents > 1 else None
         self.counters = torch.zeros(4, dtype=torch.int32, device=dev)
@@ -243,20 +360,63 @@ class DiscreteA2CAgent(A2CBase):
         t = t.to(self.device_t)
         return t if dtype is None or t.dtype == dtype else t.to(dtype)
 
-    def env_reset(self):
-        o = self.vec_env.reset()
+    def _obs_rows(self, o):
+        """observations as arena rows: flat fp32, or image frames flattened in the env's layout and kept in the arena's dtype"""
         o = o['obs'] if isinstance(o, dict) else o
-        return self._to_dev(o, torch.float32).contiguous()
+        if len(self.obs_shape) == 1:
+            return self._to_dev(o, torch.float32).contiguous()
+        o = self._to_dev(o, self.obs_dtype)
+        return o.reshape(o.shape[0], -1).contiguous()
+
+    def env_reset(self):
+        return self._obs_rows(self.vec_env.reset())
 
     def env_step(self, actions):
         o, rewards, dones, infos = self.vec_env.step(actions)
-        o = o['obs'] if isinstance(o, dict) else o
-        return self._to_dev(o, torch.float32).contiguous(), self._to_dev(rewards, torch.float32), self._to_dev(dones), infos
+        return self._obs_rows(o), self._to_dev(rewards, torch.float32), self._to_dev(dones), infos
 
     # =============================================================================== forward
-    def _forward(self, x, acts_a, acts_c, M, rows_per_chunk=None, chunk_stride=0):
-        """the actor MLP into acts_a (its last entry: [value | logits], or the logits with separate trunks), the critic MLP into acts_c"""
+    @staticmethod
+    def _conv_out(g, shp):
+        C, H, W, st, pad = g
+        return (H + 2 * pad - shp[2]) // st + 1, (W + 2 * pad - shp[3]) // st + 1
+
+    def _conv_forward(self, layers, x, acts, M, rows_per_chunk, chunk_stride):
+        """acts[l] = act(conv_l(in_l)): in_0 = the observation rows (arena order, normalised), in_l = acts[l - 1]"""
         m = self.model
+        for l, lay in enumerate(layers):
+            g = m.cnn.layers[l][1]
+            if l == 0:
+                ops.conv2d_fwd(x, lay.W, lay.b, acts[0], g, lay.act, M, nhwc=m.cnn.nhwc, rows_per_chunk=rows_per_chunk,
+                               chunk_stride=chunk_stride, x_ld=m.D, norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
+            else:
+                ops.conv2d_fwd(acts[l - 1], lay.W, lay.b, acts[l], g, lay.act, M)
+
+    def _conv_backward(self, layers, x, acts, grads, M, rows_per_chunk, chunk_stride):
+        """grads[-1] = dL/d(pre-activation of the last conv) in; weight gradients into the leading columns of `part`"""
+        m, P = self.model, self.model.num_params
+        for l in range(len(layers) - 1, -1, -1):
+            lay, g = layers[l], m.cnn.layers[l][1]
+            if l == 0:
+                ops.conv2d_bwd_weight(grads[0], x, self.part[0, lay.w_off:], self.part[0, lay.b_off:], lay.W.shape, g, self.conv_splits, M, P,
+                                      nhwc=m.cnn.nhwc, rows_per_chunk=rows_per_chunk, chunk_stride=chunk_stride, x_ld=m.D,
+                                      norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
+            else:
+                ops.conv2d_bwd_weight(grads[l], acts[l - 1], self.part[0, lay.w_off:], self.part[0, lay.b_off:], lay.W.shape, g,
+                                      self.conv_splits, M, P)
+                ops.conv2d_bwd_data(grads[l], lay.W, acts[l - 1], grads[l - 1], g, layers[l - 1].act, M)
+
+    def _forward(self, x, acts_a, acts_c, M, rows_per_chunk=None, chunk_stride=0, conv=(None, None)):
+        """the actor MLP into acts_a (its last entry: [value | logits], or the logits with separate trunks), the critic MLP into acts_c;
+        with a cnn, each MLP reads its conv trunk's output (conv = (actor conv activations, critic conv activations))"""
+        m = self.model
+        if m.cnn:
+            self._conv_forward(m.actor_conv, x, conv[0], M, rows_per_chunk, chunk_stride)
+            layerwise.forward(self.kernels, m.actor_mlp, conv[0][-1].view(M, -1), acts_a, M, m.mlp_in)
+            if m.separate:
+                self._conv_forward(m.critic_conv, x, conv[1], M, rows_per_chunk, chunk_stride)
+                layerwise.forward(self.kernels, m.critic_mlp, conv[1][-1].view(M, -1), acts_c, M, m.mlp_in)
+            return
         layerwise.forward(self.kernels, m.actor_mlp, x, acts_a, M, m.D, rows_per_chunk, chunk_stride, self.obs_norm)
         if m.separate:
             layerwise.forward(self.kernels, m.critic_mlp, x, acts_c, M, m.D, rows_per_chunk, chunk_stride, self.obs_norm)
@@ -275,7 +435,7 @@ class DiscreteA2CAgent(A2CBase):
             if self.use_action_masks:          # a2c_common.py:995-997
                 masks = self._to_dev(self.vec_env.get_action_masks()).to(torch.uint8).contiguous()
                 self.action_masks[t].copy_(masks)
-            self._forward(obs, self.r_a, self.r_c, N)
+            self._forward(obs, self.r_a, self.r_c, N, conv=(self.r_ka, self.r_kc))
             lg, ld, vl, vld = self.r_out
             ops.categorical_sample(lg, ld, K, vl, vld, masks, None if u is None else u[t].contiguous(), self.rng_seed, self.rng_epoch, t,
                                    None if vm is None else vm.running_mean, None if vm is None else vm.running_var, self.normalize_value,
@@ -293,7 +453,7 @@ class DiscreteA2CAgent(A2CBase):
             elif getattr(self.algo_observer, 'wants_infos', False):
                 self.algo_observer.process_infos(infos, None)
         # get_values (a2c_common.py:603-626): the reference's forward samples here too; only the value is used
-        self._forward(self.obs, self.r_a, self.r_c, N)
+        self._forward(self.obs, self.r_a, self.r_c, N, conv=(self.r_ka, self.r_kc))
         lg, ld, vl, vld = self.r_out
         ops.categorical_sample(None, ld, K, vl, vld, None, None, 0, None, 0, None if vm is None else vm.running_mean,
                                None if vm is None else vm.running_var, self.normalize_value, None, None, self.last_values, None, None,
@@ -329,9 +489,12 @@ class DiscreteA2CAgent(A2CBase):
         x = self.obses[0, e0:]
         if self.normalize_input:      # set_train() re-arms the obs normaliser before every minibatch (see oracle/ppo_oracle.py)
             r = m.running_mean_std
-            ops.moments_update(x, m.D, epm, H, N, r.running_mean, r.running_var, r.count, r.mean_f32, r.std_f32, self.mom_scratch,
-                               self.counters[1:2])
-        self._forward(x, self.t_a, self.t_c, mb, rows_per_chunk=epm, chunk_stride=N)
+            if self.obs_dtype == torch.uint8:
+                ops.moments_update_u8(x, m.D, epm, H, N, r.running_mean, r.running_var, r.count, r.mean_f32, r.std_f32)
+            else:
+                ops.moments_update(x, m.D, epm, H, N, r.running_mean, r.running_var, r.count, r.mean_f32, r.std_f32, self.mom_scratch,
+                                   self.counters[1:2])
+        self._forward(x, self.t_a, self.t_c, mb, rows_per_chunk=epm, chunk_stride=N, conv=(self.t_ka, self.t_kc))
         lg, ld, vl, vld = self.t_out
         d_lg, d_ld, d_vl, d_vld = self.d_out
         cfg = ops.CatLossCfg(float(self.e_clip), float(self.critic_coef), float(self.entropy_coef), int(bool(self.clip_value)),
@@ -344,11 +507,24 @@ class DiscreteA2CAgent(A2CBase):
         stats = self.loss_partials[:nb, :4].sum(dim=0).float()
         if self.diag_on:            # (sum mask, sum mask * clipped) of the minibatch: its clip fraction for diagnostics/clip_frac
             self._diag_clip.append(self.loss_partials[:nb, 4:6].sum(dim=0))
-        # ---- backward through the MLP(s): split partial gradients, then one reduction ----
-        layerwise.backward(self.kernels, m.actor_mlp, x, self.t_a, self.d_a, self.part, P, S, mb, m.D, epm, N, self.obs_norm)
-        if m.separate:
-            layerwise.backward(self.kernels, m.critic_mlp, x, self.t_c, self.d_c, self.part, P, S, mb, m.D, epm, N, self.obs_norm)
-        ops.reduce_splits(self.part, self.grad, P, S, split_stride=P)
+        # ---- backward through the MLP(s) [and the conv trunks]: split partial gradients, then one reduction ----
+        if m.cnn:
+            trunks = [(m.actor_mlp, m.actor_conv, self.t_a, self.d_a, self.t_ka, self.d_ka)]
+            if m.separate:
+                trunks.append((m.critic_mlp, m.critic_conv, self.t_c, self.d_c, self.t_kc, self.d_kc))
+            for mlp, conv, acts, grads, kacts, kgrads in trunks:
+                # dL/d(conv output) times the conv activation's derivative: the last conv's pre-activation gradient
+                layerwise.backward(self.kernels, mlp, kacts[-1].view(mb, -1), acts, grads, self.part, P, S, mb, m.mlp_in,
+                                   dx_out=kgrads[-1].view(mb, -1), dx_act=m.cnn.act)
+                self._conv_backward(conv, x, kacts, kgrads, mb, epm, N)
+            Pc = m.conv_params
+            ops.reduce_splits(self.part, self.grad, Pc, self.conv_splits, split_stride=P)
+            ops.reduce_splits(self.part[0, Pc:], self.grad[Pc:], P - Pc, S, split_stride=P)
+        else:
+            layerwise.backward(self.kernels, m.actor_mlp, x, self.t_a, self.d_a, self.part, P, S, mb, m.D, epm, N, self.obs_norm)
+            if m.separate:
+                layerwise.backward(self.kernels, m.critic_mlp, x, self.t_c, self.d_c, self.part, P, S, mb, m.D, epm, N, self.obs_norm)
+            ops.reduce_splits(self.part, self.grad, P, S, split_stride=P)
         if self.multi_gpu:          # a2c_common.py:493-509 (the Adam kernel applies the 1/world scale)
             dist.all_reduce(self.grad, op=dist.ReduceOp.SUM)
         ops.adam_step(m.flat, self.grad, m.exp_avg, m.exp_avg_sq, self.opt_state, None, self.opt_cfg, self.adam_stats, self.counters[2:3],

@@ -461,6 +461,46 @@ __global__ void __launch_bounds__(1024) explained_variance_kernel(const float* _
     }
 }
 
+// ---- obs moments of uint8 frames (x * 1/255, a2c_common.py:972-983): one CTA owns 32 columns over every row -------------------
+// block = 32 columns x 8 row lanes; the lanes' shifted sums meet in shared memory in a fixed order, so the merged statistics are
+// deterministic without cross-CTA partials (an image row has tens of thousands of columns: per-CTA partials would cost
+// n_blocks * 2 * D doubles).  The count moves in moments_u8_count_kernel, after every CTA has read the old one.
+__global__ void __launch_bounds__(256) moments_u8_kernel(
+    const uint8_t* __restrict__ x, int D, int rows_per_chunk, int n_chunks, int64_t chunk_stride,
+    double* mean, double* var, const int64_t* count, float* mean_f32, float* std_f32, float eps) {
+    __shared__ double sm[8][2][32];
+    const int c = threadIdx.x & 31, g = threadIdx.x >> 5;
+    const int col = blockIdx.x * 32 + c;
+    double s = 0.0, q = 0.0;
+    const float shift = col < D ? (float)mean[col] : 0.f;
+    if (col < D) {
+        for (int ch = 0; ch < n_chunks; ++ch) {
+            const uint8_t* base = x + (int64_t)ch * chunk_stride * D + col;
+            for (int r = g; r < rows_per_chunk; r += 8) {
+                const double d = (double)__fsub_rn(__fdiv_rn((float)__ldg(base + (int64_t)r * D), 255.0f), shift);
+                s += d; q += d * d;
+            }
+        }
+    }
+    sm[g][0][c] = s;
+    sm[g][1][c] = q;
+    __syncthreads();
+    if (g != 0 || col >= D) return;
+    double ss = 0.0, qq = 0.0;
+    for (int gg = 0; gg < 8; ++gg) { ss += sm[gg][0][c]; qq += sm[gg][1][c]; }
+    const double n = (double)rows_per_chunk * n_chunks;
+    const double ms = ss / n;
+    const double bm = (double)shift + ms;
+    const double bv = fmax(qq / n - ms * ms, 0.0);
+    double m = mean[col], v = var[col], cf = (double)count[0];
+    chan_merge(m, v, cf, bm, bv, n);
+    mean[col] = m; var[col] = v;
+    mean_f32[col] = (float)m;
+    std_f32[col] = __fsqrt_rn(__fadd_rn((float)v, eps));
+}
+
+__global__ void moments_u8_count_kernel(int64_t* count, int64_t n) { count[0] += n; }
+
 }  // namespace
 
 #ifdef B200RL_TEST_HOOKS   // test-only host entry point: compiled into tests/libb200rl_testhooks.so (csrc/build.py), not into the product library
@@ -589,6 +629,19 @@ B200RL_EXPORT int b200rl_moments_update_f64(const float* x, int D, int rows_per_
     moments_partial_kernel<<<grid, 256, smem, as_stream(stream)>>>(x, D, rows_per_chunk, chunk_stride, mean, scratch, counter,
                                                                    mean, var, count, mean_f32, std_f32, eps,
                                                                    rows_per_chunk * n_chunks);
+    B200RL_LAUNCH_CHECK();
+    return B200RL_OK;
+}
+
+B200RL_EXPORT int b200rl_moments_update_u8_f64(const uint8_t* x, int D, int rows_per_chunk, int n_chunks, int64_t chunk_stride,
+                                               double* mean, double* var, int64_t* count, float* mean_f32, float* std_f32, float eps,
+                                               void* stream) {
+    if (!x || !mean || !var || !count || !mean_f32 || !std_f32 || D <= 0 || rows_per_chunk <= 0 || n_chunks <= 0) return B200RL_EINVAL;
+    if (n_chunks > 1 && chunk_stride < rows_per_chunk) return B200RL_EINVAL;
+    cudaStream_t s = as_stream(stream);
+    moments_u8_kernel<<<(D + 31) / 32, 256, 0, s>>>(x, D, rows_per_chunk, n_chunks, chunk_stride, mean, var, count, mean_f32, std_f32, eps);
+    B200RL_LAUNCH_CHECK();
+    moments_u8_count_kernel<<<1, 1, 0, s>>>(count, (int64_t)rows_per_chunk * n_chunks);
     B200RL_LAUNCH_CHECK();
     return B200RL_OK;
 }

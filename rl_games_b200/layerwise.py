@@ -48,9 +48,10 @@ def forward(k, layers, x, acts, M, x_ld, rows_per_chunk=None, chunk_stride=0, no
 
 
 def backward(k, layers, x, acts, grads, part, split_stride, n_splits, M, x_ld, rows_per_chunk=None, chunk_stride=0, norm=(None, None),
-             dx_out=None, weights=True):
+             dx_out=None, weights=True, dx_act=0):
     """grads[l] = dL/d(pre-activation of layer l); the caller fills grads[-1], the others are overwritten.  Weight gradients go to
-    `n_splits` split rows of `part` (row stride `split_stride`) unless weights=False; with dx_out, dL/d(input) goes there."""
+    `n_splits` split rows of `part` (row stride `split_stride`) unless weights=False; with dx_out, dL/d(input) goes there, times the
+    derivative of activation `dx_act` when the input x is the (dense) output of that activation."""
     for l in range(len(layers) - 1, -1, -1):
         lay = layers[l]
         if weights:
@@ -64,4 +65,4 @@ def backward(k, layers, x, acts, grads, part, split_stride, n_splits, M, x_ld, r
         if l > 0:
             k.bwd_data(grads[l], lay.W, acts[l - 1], grads[l - 1], layers[l - 1].act, M=M)
         elif dx_out is not None:
-            k.bwd_data(grads[0], lay.W, None, dx_out, 0, M=M)
+            k.bwd_data(grads[0], lay.W, x if dx_act else None, dx_out, dx_act, M=M)

@@ -234,6 +234,46 @@ def linear_bwd_weight_tc(dY, X, dW_part, db_part, K, Nout, n_splits, rows_per_ch
           'linear_bwd_weight_tc')
 
 
+def _conv_src(X):
+    """(x_u8) of a conv input: uint8 frames or fp32 rows"""
+    if X.dtype not in (torch.uint8, torch.float32):
+        raise TypeError(f'conv2d input dtype {X.dtype}: uint8 or float32')
+    return int(X.dtype == torch.uint8)
+
+
+def conv2d_fwd(X, W, b, Y, geo, act, M, nhwc=False, rows_per_chunk=None, chunk_stride=0, x_ld=None, norm_mean=None, norm_std=None):
+    """Y[M, Cout, Ho, Wo] = act(conv(norm(X)) + b); geo = (C, H, W, stride, pad) of the input, W: [Cout, C, KH, KW]"""
+    C, H, Wd, st, pad = geo
+    Cout, _, KH, KW = W.shape
+    check(lib.b200rl_conv2d_fwd_f32(ptr(X), _conv_src(X), int(nhwc), M if rows_per_chunk is None else rows_per_chunk, chunk_stride,
+                                    C * H * Wd if x_ld is None else x_ld, ptr(norm_mean), ptr(norm_std), ptr(W), ptr(b), ptr(Y), M, C, H,
+                                    Wd, Cout, KH, KW, st, pad, act, _stream()), 'conv2d_fwd')
+
+
+def conv2d_bwd_data(dY, W, A_prev, dX, geo, act_prev, M):
+    """dX[M, C, H, W] = conv^T(dY, W) * act'(A_prev)"""
+    C, H, Wd, st, pad = geo
+    Cout, _, KH, KW = W.shape
+    check(lib.b200rl_conv2d_bwd_data_f32(ptr(dY), ptr(W), ptr(A_prev), ptr(dX), M, C, H, Wd, Cout, KH, KW, st, pad, act_prev, _stream()),
+          'conv2d_bwd_data')
+
+
+def conv2d_bwd_weight(dY, X, dW_part, db_part, W_shape, geo, n_splits, M, split_stride, nhwc=False, rows_per_chunk=None,
+                      chunk_stride=0, x_ld=None, norm_mean=None, norm_std=None):
+    C, H, Wd, st, pad = geo
+    Cout, _, KH, KW = W_shape
+    check(lib.b200rl_conv2d_bwd_weight_f32(ptr(dY), ptr(X), _conv_src(X), int(nhwc), M if rows_per_chunk is None else rows_per_chunk,
+                                           chunk_stride, C * H * Wd if x_ld is None else x_ld, ptr(norm_mean), ptr(norm_std), ptr(dW_part),
+                                           ptr(db_part), split_stride, M, C, H, Wd, Cout, KH, KW, st, pad, n_splits, _stream()),
+          'conv2d_bwd_weight')
+
+
+def moments_update_u8(x, D, rows_per_chunk, n_chunks, chunk_stride, mean, var, count, mean_f32, std_f32, eps=1e-5):
+    """moments_update of uint8 rows, read as x / 255"""
+    check(lib.b200rl_moments_update_u8_f64(ptr(x), D, rows_per_chunk, n_chunks, chunk_stride, ptr(mean), ptr(var), ptr(count),
+                                           ptr(mean_f32), ptr(std_f32), eps, _stream()), 'moments_update_u8')
+
+
 def reduce_splits(part, out, n, n_splits, split_stride=None):
     check(lib.b200rl_reduce_splits_f32(ptr(part), ptr(out), n, n_splits, n if split_stride is None else split_stride,
                                        _stream()), 'reduce_splits')
