@@ -181,6 +181,20 @@ int b200rl_conv2d_bwd_weight_f32(const float* dY, const void* X, int x_u8, int x
                                  int64_t x_ld, const float* norm_mean, const float* norm_std, float* dW_part, float* db_part,
                                  int64_t split_stride, int M, int C, int H, int Wd, int Cout, int KH, int KW, int stride, int pad,
                                  int n_splits, void* stream);
+/* The same three convolutions on the tensor cores (conv_tc.cu: wgmma implicit GEMMs, operands rounded to bf16 while they are staged,
+ * fp32 accumulate in registers, fp32 bias / activation / outputs): the mixed_precision path.  Same arguments and semantics as the
+ * _f32 functions, except that the weights are W_bf16 (required): the filters [Cout, C, KH, KW] in PyTorch's layout as bf16, e.g.
+ * their slice of b200rl_cast_bf16's copy of the flat parameter arena.  B200RL_EUNSUPPORTED: more than 2^31 - 1 tiles of 128 output
+ * rows, more than 65535 column tiles or splits. */
+int b200rl_conv2d_fwd_tc(const void* X, int x_u8, int x_nhwc, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
+                         const float* norm_mean, const float* norm_std, const void* W_bf16, const float* b, float* Y,
+                         int M, int C, int H, int Wd, int Cout, int KH, int KW, int stride, int pad, int act, void* stream);
+int b200rl_conv2d_bwd_data_tc(const float* dY, const void* W_bf16, const float* A_prev, float* dX, int M, int C, int H, int Wd,
+                              int Cout, int KH, int KW, int stride, int pad, int act_prev, void* stream);
+int b200rl_conv2d_bwd_weight_tc(const float* dY, const void* X, int x_u8, int x_nhwc, int rows_per_chunk, int64_t chunk_stride,
+                                int64_t x_ld, const float* norm_mean, const float* norm_std, float* dW_part, float* db_part,
+                                int64_t split_stride, int M, int C, int H, int Wd, int Cout, int KH, int KW, int stride, int pad,
+                                int n_splits, void* stream);
 /* out[i] = sum_s part[s*split_stride + i]  (deterministic, fixed order) */
 /* The same three building blocks on the tensor cores (wgmma, bf16 operands rounded while they are staged, fp32 accumulate in
  * registers, fp32 bias / activation / outputs) for ANY layer width: the mixed_precision path of LSTM gate GEMMs and of MLPs the fused

@@ -8,6 +8,10 @@ STATUS: parity-green on an H100 (``tests/test_discrete_gpu.py``) against a CPU o
 mask_inv_counts (stats.cu, gae.cu), post_step (rollout.cu), adam_step (adam.cu).
 
 Image observations (``cnn: {type: conv2d}`` on a rank-3 Box) run a conv trunk (csrc/conv.cu) in front of the MLP; see DESIGN.md §4.
+Precision is read by value: ``mixed_precision: True`` runs every conv and linear layer of the rollout and the update on the bf16
+tensor cores (csrc/conv_tc.cu, csrc/gemm_tc.cu; the categorical head kernels stay fp32), with the weights read from ``wbf``, a bf16
+twin of the parameter arena refreshed after every optimiser step, weight load and weight broadcast; ``False`` or no key runs the fp32
+kernels above.
 Scope of this first edition: one GPU, eager launches (no CUDA graph), flat Box observations or conv2d frames, ``Discrete(K)`` or multi-discrete
 ``Tuple(Discrete(K_j))`` action spaces (K_j <= 64, <= 8 heads), no RNN, no central value.  The scheduler steps once per MINI-EPOCH on the mean KL like the reference
 (a2c_common.py:1265-1272), which costs one host sync per mini-epoch.
@@ -272,6 +276,8 @@ class DiscreteA2CAgent(A2CBase):
         if max(self.head_sizes or [self.actions_num]) > 64:
             raise NotImplementedError('more than 64 actions in one discrete head')
         self.use_action_masks = bool(config.get('use_action_masks', False))
+        # True: every conv and linear layer on the bf16 tensor cores (conv_tc.cu, gemm_tc.cu); False or absent: the fp32 kernels
+        self.mixed_precision = bool(config.get('mixed_precision') or False)
 
     def _make_writer(self):
         return make_summary_writer(self.summaries_dir)          # on every rank
@@ -319,7 +325,15 @@ class DiscreteA2CAgent(A2CBase):
         else:
             self.r_c = self.t_c = self.d_c = None
             self.r_out, self.t_out, self.d_out = ((a[-1][:, 1:], K + 1, a[-1], K + 1) for a in (self.r_a, self.t_a, self.d_a))
-        self.n_splits = layerwise.n_splits(mb)
+        if self.mixed_precision:
+            # tensor-core weight gradients: a CTA owns a [128 x <=128] tile of dW and a row split; the continuous agent's layer-wise
+            # rule (16 splits at most) keeps enough CTAs per layer while the split partials stay small
+            self.n_splits = max(1, min(16, mb // 512))
+            self.wbf = torch.empty(m.num_params, dtype=torch.bfloat16, device=dev)     # bf16 twin of the parameter arena (weight operands)
+            ops.cast_bf16(m.flat, self.wbf)
+        else:
+            self.n_splits = layerwise.n_splits(mb)
+            self.wbf = None
         if m.cnn:
             # conv activations (NCHW rows) of each trunk, rollout / training, and their gradients (pre-activation); the conv weight
             # gradients split over the output pixels' rows, so they take more split rows than the MLP (the leading conv_params columns)
@@ -351,7 +365,9 @@ class DiscreteA2CAgent(A2CBase):
         self.shaper_cfg = ops.ShaperCfg(float(rs.scale_value), float(rs.shift_value), float(rs.min_val), float(rs.max_val),
                                         float(self.gamma), int(bool(rs.log_val)), int(bool(self.value_bootstrap)))
         self.obs_norm = _RunningStats.f32_pair(m.running_mean_std)
-        self.kernels = layerwise.Kernels()
+        # every conv and linear layer of the rollout and the update runs on one precision: fp32 CUDA cores, or bf16 tensor cores with
+        # the weights read from the twin (the categorical head kernels stay fp32 either way)
+        self.kernels = layerwise.Kernels(tc=True, bf16_arena=(m.flat, self.wbf)) if self.mixed_precision else layerwise.Kernels()
         self._tensors_ready = True
 
     # =============================================================================== env plumbing (tensor envs on the device)
@@ -387,24 +403,25 @@ class DiscreteA2CAgent(A2CBase):
         for l, lay in enumerate(layers):
             g = m.cnn.layers[l][1]
             if l == 0:
-                ops.conv2d_fwd(x, lay.W, lay.b, acts[0], g, lay.act, M, nhwc=m.cnn.nhwc, rows_per_chunk=rows_per_chunk,
-                               chunk_stride=chunk_stride, x_ld=m.D, norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
+                self.kernels.conv_fwd(x, lay.W, lay.b, acts[0], g, lay.act, M, nhwc=m.cnn.nhwc, rows_per_chunk=rows_per_chunk,
+                                      chunk_stride=chunk_stride, x_ld=m.D, norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
             else:
-                ops.conv2d_fwd(acts[l - 1], lay.W, lay.b, acts[l], g, lay.act, M)
+                self.kernels.conv_fwd(acts[l - 1], lay.W, lay.b, acts[l], g, lay.act, M)
 
     def _conv_backward(self, layers, x, acts, grads, M, rows_per_chunk, chunk_stride):
         """grads[-1] = dL/d(pre-activation of the last conv) in; weight gradients into the leading columns of `part`"""
         m, P = self.model, self.model.num_params
         for l in range(len(layers) - 1, -1, -1):
             lay, g = layers[l], m.cnn.layers[l][1]
+            k = self.kernels
             if l == 0:
-                ops.conv2d_bwd_weight(grads[0], x, self.part[0, lay.w_off:], self.part[0, lay.b_off:], lay.W.shape, g, self.conv_splits, M, P,
-                                      nhwc=m.cnn.nhwc, rows_per_chunk=rows_per_chunk, chunk_stride=chunk_stride, x_ld=m.D,
-                                      norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
+                k.conv_bwd_weight(grads[0], x, self.part[0, lay.w_off:], self.part[0, lay.b_off:], lay.W.shape, g, self.conv_splits, M, P,
+                                  nhwc=m.cnn.nhwc, rows_per_chunk=rows_per_chunk, chunk_stride=chunk_stride, x_ld=m.D,
+                                  norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
             else:
-                ops.conv2d_bwd_weight(grads[l], acts[l - 1], self.part[0, lay.w_off:], self.part[0, lay.b_off:], lay.W.shape, g,
-                                      self.conv_splits, M, P)
-                ops.conv2d_bwd_data(grads[l], lay.W, acts[l - 1], grads[l - 1], g, layers[l - 1].act, M)
+                k.conv_bwd_weight(grads[l], acts[l - 1], self.part[0, lay.w_off:], self.part[0, lay.b_off:], lay.W.shape, g,
+                                  self.conv_splits, M, P)
+                k.conv_bwd_data(grads[l], lay.W, acts[l - 1], grads[l - 1], g, layers[l - 1].act, M)
 
     def _forward(self, x, acts_a, acts_c, M, rows_per_chunk=None, chunk_stride=0, conv=(None, None)):
         """the actor MLP into acts_a (its last entry: [value | logits], or the logits with separate trunks), the critic MLP into acts_c;
@@ -529,7 +546,13 @@ class DiscreteA2CAgent(A2CBase):
             dist.all_reduce(self.grad, op=dist.ReduceOp.SUM)
         ops.adam_step(m.flat, self.grad, m.exp_avg, m.exp_avg_sq, self.opt_state, None, self.opt_cfg, self.adam_stats, self.counters[2:3],
                       n=P)
+        self._repack()
         return stats
+
+    def _repack(self):
+        """the bf16 twin follows the fp32 arena: after every optimiser step, weight load and multi-GPU weight broadcast"""
+        if getattr(self, 'wbf', None) is not None:
+            ops.cast_bf16(self.model.flat, self.wbf)
 
     def train_epoch(self, u=None):
         """DiscreteA2CBase.train_epoch (a2c_common.py:1233-1289): returns the reference's tuple."""
@@ -580,6 +603,10 @@ class DiscreteA2CAgent(A2CBase):
         return super().train()
 
     # =============================================================================== weights / checkpoints (a2c_common.py:825-921)
+    def set_weights(self, weights):
+        super().set_weights(weights)
+        self._repack()
+
     def get_full_state_weights(self):
         self.init_tensors()
         state = self.get_weights()

@@ -25,17 +25,22 @@ def n_splits(M):
 
 
 class Kernels:
-    """The three layer GEMMs of one precision: fp32, or the tensor cores with weight operands read from a bf16 twin of the fp32
-    arena, ``bf16_arena = (fp32 arena, bf16 arena)``, in the forward and the data gradient.  The ``ops`` functions are looked up
-    when the set is built, so that a substitute installed on ``ops`` before an agent is built is what runs."""
+    """The three layer GEMMs of one precision, and the three convolutions of an image trunk: fp32, or the tensor cores with weight
+    operands read from a bf16 twin of the fp32 arena, ``bf16_arena = (fp32 arena, bf16 arena)``, in the forward and the data gradient
+    (the tensor-core convs need the twin).  The ``ops`` functions are looked up when the set is built, so that a substitute installed on
+    ``ops`` before an agent is built is what runs."""
 
     def __init__(self, tc=False, bf16_arena=None):
         if not tc:
             self.fwd, self.bwd_data, self.bwd_weight = ops.linear_fwd, ops.linear_bwd_data, ops.linear_bwd_weight
+            self.conv_fwd, self.conv_bwd_data, self.conv_bwd_weight = ops.conv2d_fwd, ops.conv2d_bwd_data, ops.conv2d_bwd_weight
             return
         self.fwd = functools.partial(ops.linear_fwd_tc, bf16_arena=bf16_arena)
         self.bwd_data = functools.partial(ops.linear_bwd_data_tc, bf16_arena=bf16_arena)
         self.bwd_weight = ops.linear_bwd_weight_tc
+        self.conv_fwd = functools.partial(ops.conv2d_fwd_tc, bf16_arena=bf16_arena)
+        self.conv_bwd_data = functools.partial(ops.conv2d_bwd_data_tc, bf16_arena=bf16_arena)
+        self.conv_bwd_weight = ops.conv2d_bwd_weight_tc
 
 
 def forward(k, layers, x, acts, M, x_ld, rows_per_chunk=None, chunk_stride=0, norm=(None, None)):

@@ -268,6 +268,41 @@ def conv2d_bwd_weight(dY, X, dW_part, db_part, W_shape, geo, n_splits, M, split_
           'conv2d_bwd_weight')
 
 
+def _conv_bf16_ptr(W, bf16_arena):
+    """the bf16 twin of conv filters W (a view of bf16_arena's fp32 arena): the tensor-core convs read no fp32 weights"""
+    p = _bf16_view_ptr(W, bf16_arena)
+    if p is None:
+        raise B200RLError('conv2d_*_tc: W must be a contiguous view of the fp32 arena of bf16_arena = (fp32 arena, bf16 twin)')
+    return p
+
+
+def conv2d_fwd_tc(X, W, b, Y, geo, act, M, nhwc=False, rows_per_chunk=None, chunk_stride=0, x_ld=None, norm_mean=None, norm_std=None,
+                  bf16_arena=None):
+    """conv2d_fwd on the tensor cores (bf16 operands, fp32 accumulate); weights from the bf16 twin"""
+    C, H, Wd, st, pad = geo
+    Cout, _, KH, KW = W.shape
+    check(lib.b200rl_conv2d_fwd_tc(ptr(X), _conv_src(X), int(nhwc), M if rows_per_chunk is None else rows_per_chunk, chunk_stride,
+                                   C * H * Wd if x_ld is None else x_ld, ptr(norm_mean), ptr(norm_std), _conv_bf16_ptr(W, bf16_arena), ptr(b),
+                                   ptr(Y), M, C, H, Wd, Cout, KH, KW, st, pad, act, _stream()), 'conv2d_fwd_tc')
+
+
+def conv2d_bwd_data_tc(dY, W, A_prev, dX, geo, act_prev, M, bf16_arena=None):
+    C, H, Wd, st, pad = geo
+    Cout, _, KH, KW = W.shape
+    check(lib.b200rl_conv2d_bwd_data_tc(ptr(dY), _conv_bf16_ptr(W, bf16_arena), ptr(A_prev), ptr(dX), M, C, H, Wd, Cout, KH, KW, st, pad,
+                                        act_prev, _stream()), 'conv2d_bwd_data_tc')
+
+
+def conv2d_bwd_weight_tc(dY, X, dW_part, db_part, W_shape, geo, n_splits, M, split_stride, nhwc=False, rows_per_chunk=None,
+                         chunk_stride=0, x_ld=None, norm_mean=None, norm_std=None):
+    C, H, Wd, st, pad = geo
+    Cout, _, KH, KW = W_shape
+    check(lib.b200rl_conv2d_bwd_weight_tc(ptr(dY), ptr(X), _conv_src(X), int(nhwc), M if rows_per_chunk is None else rows_per_chunk,
+                                          chunk_stride, C * H * Wd if x_ld is None else x_ld, ptr(norm_mean), ptr(norm_std), ptr(dW_part),
+                                          ptr(db_part), split_stride, M, C, H, Wd, Cout, KH, KW, st, pad, n_splits, _stream()),
+          'conv2d_bwd_weight_tc')
+
+
 def moments_update_u8(x, D, rows_per_chunk, n_chunks, chunk_stride, mean, var, count, mean_f32, std_f32, eps=1e-5):
     """moments_update of uint8 rows, read as x / 255"""
     check(lib.b200rl_moments_update_u8_f64(ptr(x), D, rows_per_chunk, n_chunks, chunk_stride, ptr(mean), ptr(var), ptr(count),

@@ -2,14 +2,16 @@
 steps of 4x84x84 uint8 frames from a synthetic device env, 6 actions, Nature-CNN trunk (32@8/4, 64@4/2, 64@3/1, elu), MLP [512],
 minibatch 2048 x 4 mini-epochs, input normaliser on.
 
-Prints one JSON line:
-- epoch_ms: one train_epoch (rollout + GAE + 16 minibatch updates), CUDA events, after a warm-up epoch (median of --epochs);
-- mb_update_ms: one minibatch update of the agent (forward, loss, backward, Adam);
+Two arms in one process, alternated round by round: the fp32 agent (mixed_precision: False, conv.cu + mlp_simt.cu) and the
+tensor-core agent (mixed_precision: True, conv_tc.cu + gemm_tc.cu).  Prints one JSON line:
+- epoch_ms / mb_update_ms per arm: one train_epoch (rollout + GAE + 16 minibatch updates) and one minibatch update (forward, loss,
+  backward, Adam), CUDA events, after a warm-up epoch: the median over --rounds rounds and the [min, max] spread;
 - ref_fp32_ms / ref_bf16_ms: the reference's ModelA2C network (oracle/_ref) on the same 2048 frames: forward, the same kind of loss,
   backward and torch Adam, in fp32 and under bf16 autocast (cuDNN);
-- conv_share: the conv kernels' share of the GPU kernel time of one epoch, from a separate torch.profiler run;
-- the card's name and power limit.
-Usage: python tools/cnn_ab.py [--epochs 3]"""
+- conv_share per arm: the conv kernels' share of the GPU kernel time of one epoch, from a separate torch.profiler run;
+- max_abs_diff: the largest difference in logits and in value between the arms on the same frames with the same weights;
+- the card's name and power limit, read in the same call.
+Usage: python tools/cnn_ab.py [--rounds 5]"""
 import argparse
 import json
 import os
@@ -53,14 +55,14 @@ class FrameEnv:
         return {'observation_space': Box(0, 255, FRAME, 'uint8'), 'action_space': Discrete(K)}
 
 
-def make_agent():
+def make_agent(mixed_precision):
     from rl_games_b200.runner import Runner
     env = FrameEnv()
     config = {'name': 'cnn_ab', 'env_name': 'unused', 'reward_shaper': {'min_val': -1, 'max_val': 1}, 'normalize_value': True,
               'normalize_input': True, 'normalize_advantage': True, 'gamma': 0.99, 'tau': 0.95, 'learning_rate': 3e-4, 'grad_norm': 1.0,
               'entropy_coef': 0.01, 'truncate_grads': True, 'e_clip': 0.2, 'clip_value': True, 'num_actors': N, 'horizon_length': H,
               'minibatch_size': MB, 'mini_epochs': 4, 'critic_coef': 1, 'lr_schedule': None, 'kl_threshold': 0.008, 'device': DEV,
-              'mixed_precision': False, 'max_epochs': 1000, 'save_frequency': 0, 'print_stats': False,
+              'mixed_precision': mixed_precision, 'max_epochs': 1000, 'save_frequency': 0, 'print_stats': False,
               'train_dir': tempfile.mkdtemp(prefix='cnn_ab_'), 'env_info': env.get_env_info(), 'vec_env': env}
     r = Runner()
     r.load({'params': {'seed': 1, 'algo': {'name': 'a2c_discrete'}, 'model': {'name': 'discrete_a2c'}, 'network': NETWORK, 'config': config}})
@@ -110,32 +112,66 @@ def card():
     return q.strip().splitlines()[0] if q.strip() else torch.cuda.get_device_name(0)
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--epochs', type=int, default=3)
-    args = ap.parse_args()
-    assert torch.cuda.is_available(), 'cnn_ab measures on a GPU'
-    torch.cuda.set_device(0)
-    agent = make_agent()
-    agent.train_epoch()                                    # warm-up: every shape of the timed window
-    epoch_ms = timed(agent.train_epoch, args.epochs)
-    mb_ms = timed(lambda: agent._minibatch_update(0), 10)
-    frames = agent.obses.view(H * N, -1)[:MB].view(MB, *FRAME)
-    ref32, ref16 = reference_ms(frames, False, 10), reference_ms(frames, True, 10)
+def conv_share(agent):
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         agent.train_epoch()
         torch.cuda.synchronize()
     tot = conv = 0.0
+    per = []
     for e in prof.key_averages():
         t = getattr(e, 'device_time_total', None) or getattr(e, 'cuda_time_total', 0.0)
         if e.key.startswith(('cuda', 'Memcpy', 'Memset')) or t <= 0:
             continue
         tot += t
-        conv += t if 'conv2d_' in e.key else 0.0
-    print(json.dumps({'workload': 'pong-shaped: 64x128 uint8 4x84x84, nature-cnn + [512], mb 2048 x 4', 'epoch_ms': round(epoch_ms, 2),
-                      'mb_update_ms': round(mb_ms, 3), 'ref_fp32_mb_ms': round(ref32, 3), 'ref_bf16_autocast_mb_ms': round(ref16, 3),
-                      'conv_share_of_kernel_time': round(conv / max(tot, 1e-9), 3), 'card': card()}))
+        conv += t if ('conv2d_' in e.key or 'conv_tc_' in e.key) else 0.0
+        per.append((t, e.key))
+    top = [[k[:90], round(t / 1e3, 2)] for t, k in sorted(per, reverse=True)[:6]]       # ms per epoch
+    return round(conv / max(tot, 1e-9), 3), top
+
+
+def spread(ts):
+    ts = sorted(ts)
+    return round(ts[len(ts) // 2], 3), [round(ts[0], 3), round(ts[-1], 3)]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--rounds', type=int, default=5)
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), 'cnn_ab measures on a GPU'
+    torch.cuda.set_device(0)
+    arms = {'fp32': make_agent(False), 'tc': make_agent(True)}
+    for a in arms.values():
+        a.train_epoch()                                    # warm-up: every shape of the timed window
+        a._minibatch_update(0)
+    ep = {k: [] for k in arms}
+    mb = {k: [] for k in arms}
+    for _ in range(args.rounds):                           # the arms alternate: both see the same state of the shared machine
+        for k, a in arms.items():
+            ep[k].append(timed(a.train_epoch, 1))
+            mb[k].append(timed(lambda: a._minibatch_update(0), 5))
+    a32, atc = arms['fp32'], arms['tc']
+    frames = a32.obses.view(H * N, -1)[:MB].view(MB, *FRAME)
+    ref32, ref16 = reference_ms(frames, False, 10), reference_ms(frames, True, 10)
+    share = {k: conv_share(a) for k, a in arms.items()}
+    # the same weights and frames through both arms' rollout forward
+    atc.set_weights(a32.get_weights())
+    for a in arms.values():
+        a._forward(a32.obs, a.r_a, a.r_c, N, conv=(a.r_ka, a.r_kc))
+    torch.cuda.synchronize()
+    d_logits = (a32.r_out[0] - atc.r_out[0]).abs().max().item()
+    d_value = (a32.r_out[2][:, :1] - atc.r_out[2][:, :1]).abs().max().item()
+    out = {'workload': 'pong-shaped: 64x128 uint8 4x84x84, nature-cnn + [512], mb 2048 x 4', 'rounds': args.rounds}
+    for k in arms:
+        (e, es), (m, ms) = spread(ep[k]), spread(mb[k])
+        out[k] = {'epoch_ms': e, 'epoch_ms_spread': es, 'mb_update_ms': m, 'mb_update_ms_spread': ms,
+                  'conv_share_of_kernel_time': share[k][0], 'top_kernels_ms_per_epoch': share[k][1]}
+    out.update({'ref_fp32_mb_ms': round(ref32, 3), 'ref_bf16_autocast_mb_ms': round(ref16, 3),
+                'max_abs_diff': {'logits': d_logits, 'value': d_value,
+                                 'logits_scale': a32.r_out[0].abs().max().item(), 'value_scale': a32.r_out[2][:, :1].abs().max().item()},
+                'card': card()})
+    print(json.dumps(out))
 
 
 if __name__ == '__main__':
