@@ -382,6 +382,13 @@ int b200rl_categorical_loss_f32(const float* logits, int ld, int K, int n_heads,
                                 int rows_per_chunk, int64_t chunk_stride, int M, const b200rl_cat_loss_cfg* cfg_host,
                                 const float* inv_count_dev, float* d_logits, int d_ld, float* d_value, int dv_ld,
                                 double* partials, int max_partials, int* n_blocks_out_host, void* stream);
+/* Deterministic categorical head of the discrete player (csrc/player.cu; algos_torch/players.py get_action / get_masked_action with
+ * is_deterministic): actions_out int64 [N, max(n_heads, 1)] = the per-head argmax of logits [N, ld] (K used; heads laid out as in
+ * b200rl_categorical_sample_f32, n_heads = 0 or NULL sizes: one head of K <= 64, else <= 8 heads of <= 64) over the actions the optional
+ * action_masks uint8 [N, K] allow.  Ties go to the lowest index and NaN wins, as torch.argmax; a head with every action masked gives 0.
+ * Caller-owned buffers, no allocation, asynchronous on `stream`, graph-capturable. */
+int b200rl_categorical_argmax_f32(const float* logits, int ld, int K, int n_heads, const int* head_sizes_host,
+                                  const uint8_t* action_masks, int64_t* actions_out, int N, void* stream);
 
 /* Central value with a multi-agent env (agents > 1; central_value.py:224-244).
  *  b200rl_cv_value_broadcast_f32: out[e*agents + a] = denorm(val[e]) for the N envs' critic values val[N] (de-normalised with the value

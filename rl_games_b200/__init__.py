@@ -14,3 +14,10 @@ def register_sac(runner):
     """rl_games_b200.runner.register_sac: the B200 SAC agent behind `sac` in the given runner's algo_factory"""
     from .runner import register_sac as _register_sac
     return _register_sac(runner)
+
+
+def register_players(runner):
+    """rl_games_b200.runner.register_players: the CUDA players behind `a2c_continuous` / `a2c_discrete` / `sac` in the given runner's
+    player_factory"""
+    from .runner import register_players as _register_players
+    return _register_players(runner)

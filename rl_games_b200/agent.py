@@ -49,6 +49,38 @@ def rescale_actions(low, high, action):
     return action * d + m
 
 
+def rollout_precision(model, actions_num, config):
+    """(fused_ok, use_tc, gemm_tc, rollout_fp32) of a continuous policy: the kernels the rollout's policy forward runs on, resolved from
+    `mixed_precision` and `b200_rollout_fp32`; the agent and the player both take them from here"""
+    # wgmma kernels: three hidden layers that fit the compiled tile widths (u1 <= 256, u2 <= 128, u3 <= 64; narrower layers are
+    # zero-padded), elu / relu / tanh, obs <= 256 (wide observations, 64 < obs <= 256: layer 1 runs in kernels of its own,
+    # l1_fwd_tc / l1_wgrad_tc), <= 15 actions; anything else runs on the fp32 kernels
+    tc_ok = model.activation in ('elu', 'relu', 'tanh') and ops.tc_supported(model.D, model.units, actions_num, True)
+    # (a fixed sigma other than the plain log-std -- a floor, bounds, 'softplus' / 'linear' -- is applied outside the kernels on the
+    #  log-std vector they read; the fused kernels take the raw parameter from the packed arena, so such policies run layer by layer.
+    #  Separate actor / critic trunks need their gradient mask applied between the split reduction and the optimiser, which the fused
+    #  tail does in one launch: layer by layer as well.  A state-dependent sigma head runs on the fp32 or the layer-wise tensor-core
+    #  kernels: the fused kernels have 16 head rows)
+    fused_ok = tc_ok and not model.is_rnn() and not getattr(model, 'sigma_transform', False) and \
+        getattr(model, 'fixed_sigma', True) and not getattr(model, 'separate', False)
+    # None (key absent) = the reference's 'auto' (a2c_common.py:427-429): the wgmma path where this build has kernels for the geometry
+    mixed_precision = config.get('mixed_precision', None)
+    if mixed_precision is None:
+        mixed_precision = fused_ok
+    # mixed_precision: True -> the fused wgmma MLP kernels where they have the geometry (use_tc), else the SAME host composition as the
+    # fp32 path with every GEMM on the tensor cores (gemm_tc: bf16 operands, fp32 accumulate -- gemm_tc.cu): LSTM policies (gate GEMMs,
+    # BPTT), MLPs wider / deeper than the fused tiles.  The reference's autocast covers nn.LSTM and nn.Linear alike (a2c_continuous.py:173).
+    use_tc = bool(mixed_precision) and fused_ok
+    gemm_tc = bool(mixed_precision) and not fused_ok
+    # Rollout precision.  The reference evaluates the policy during the rollout OUTSIDE autocast (a2c_common.py:581-600: fp32 / TF32)
+    # and only calc_gradients under bf16 autocast (a2c_continuous.py:173).  Default here: the rollout uses the same bf16 wgmma
+    # kernels as the update, so old_neglogp / old mu come from the SAME arithmetic the first mini-epoch re-evaluates (ratio == 1 at
+    # the first minibatch, which the reference's mix does not give).  b200_rollout_fp32: True restores the reference's split: fp32
+    # CUDA-core kernels for get_action_values / get_values, bf16 tensor cores for the update.
+    rollout_fp32 = use_tc and bool(config.get('b200_rollout_fp32', False))
+    return fused_ok, use_tc, gemm_tc, rollout_fp32
+
+
 class _Dataset:
     """datasets.PPODataset look-alike (datasets.py:7-95): len() minibatches, [i] -> dict of reference-layout
     COPIES of minibatch i (flat order env*H+t) tagged with its index so train_actor_critic() can run the
@@ -108,19 +140,7 @@ class A2CAgent(A2CBase):
         # hardware supports it, a2c_common.py:427-429) and resolves to the wgmma path where this build has kernels for the
         # geometry, else to fp32 (a HIGHER precision than the reference's default), saying so once.
         self.is_rnn = self.model.is_rnn()
-        # wide observations (64 < obs <= 256): layer 1 runs in kernels of its own (l1_fwd_tc / l1_wgrad_tc)
-        allow_wide = True
-        # wgmma kernels: three hidden layers that fit the compiled tile widths (u1 <= 256, u2 <= 128, u3 <= 64; narrower layers are
-        # zero-padded), elu / relu / tanh, obs <= 256, <= 15 actions; anything else runs on the fp32 kernels
-        tc_ok = self.model.activation in ('elu', 'relu', 'tanh') and \
-            ops.tc_supported(self.model.D, self.model.units, self.actions_num, allow_wide)
-        # (a fixed sigma other than the plain log-std -- a floor, bounds, 'softplus' / 'linear' -- is applied outside the kernels on the
-        #  log-std vector they read; the fused kernels take the raw parameter from the packed arena, so such policies run layer by layer.
-        #  Separate actor / critic trunks need their gradient mask applied between the split reduction and the optimiser, which the fused
-        #  tail does in one launch: layer by layer as well.  A state-dependent sigma head runs on the fp32 or the layer-wise tensor-core
-        #  kernels: the fused kernels have 16 head rows)
-        fused_ok = tc_ok and not self.is_rnn and not getattr(self.model, 'sigma_transform', False) and \
-            getattr(self.model, 'fixed_sigma', True) and not getattr(self.model, 'separate', False)
+        fused_ok, self.use_tc, self.gemm_tc, self.rollout_fp32 = rollout_precision(self.model, self.actions_num, config)
         if self.mixed_precision is None:
             self.mixed_precision = fused_ok
             if not self.mixed_precision and self.global_rank == 0:
@@ -134,21 +154,10 @@ class A2CAgent(A2CBase):
                 raise ValueError(f"Horizon length ({self.horizon_length}) must be divisible by sequence length ({self.seq_length})")
             if not self.zero_rnn_on_done:
                 raise NotImplementedError('zero_rnn_on_done: False is not on the B200 hot path')
-        # mixed_precision: True -> the fused wgmma MLP kernels where they have the geometry (use_tc), else the SAME host composition as the
-        # fp32 path with every GEMM on the tensor cores (gemm_tc: bf16 operands, fp32 accumulate -- gemm_tc.cu): LSTM policies (gate GEMMs,
-        # BPTT), MLPs wider / deeper than the fused tiles.  The reference's autocast covers nn.LSTM and nn.Linear alike (a2c_continuous.py:173).
-        self.use_tc = bool(self.mixed_precision) and fused_ok
-        self.gemm_tc = bool(self.mixed_precision) and not fused_ok
         self.obs_norm = _RunningStats.f32_pair(self.model.running_mean_std)
         # with an LSTM in front the MLP input is h (dense, not normalised)
         self.mlp_norm = (None, None) if (self.is_rnn and self.model.rnn_before_mlp) else self.obs_norm
         self.tc_wide = self.use_tc and ops.tc_kind(self.model.D, self.model.units, self.actions_num) == 2
-        # Rollout precision.  The reference evaluates the policy during the rollout OUTSIDE autocast (a2c_common.py:581-600: fp32 / TF32)
-        # and only calc_gradients under bf16 autocast (a2c_continuous.py:173).  Default here: the rollout uses the same bf16 wgmma
-        # kernels as the update, so old_neglogp / old mu come from the SAME arithmetic the first mini-epoch re-evaluates (ratio == 1 at
-        # the first minibatch, which the reference's mix does not give).  b200_rollout_fp32: True restores the reference's split: fp32
-        # CUDA-core kernels for get_action_values / get_values, bf16 tensor cores for the update.
-        self.rollout_fp32 = self.use_tc and bool(config.get('b200_rollout_fp32', False))
         if self.use_tc and config.get('b200_pipelined_wgrad', False) and (self.tc_wide or list(self.model.units) != [256, 128, 64]):
             raise NotImplementedError('b200_pipelined_wgrad is an option of the native resident-weights geometry (obs <= 64, MLP [256,128,64])')
         self.dataset = _Dataset(self)

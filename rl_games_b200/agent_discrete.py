@@ -32,6 +32,33 @@ from .layerwise import Layer
 from .model import _apply_init, check_network_params, FlatParamModel, _RunningStats
 
 
+def discrete_spaces(observation_space, action_space, network_params, config):
+    """(obs_shape, obs_dtype, head_sizes, actions_num, is_multi_discrete, mixed_precision) of a discrete policy, or the refusal of its
+    spaces; the agent and the player both take them from here"""
+    # flat Box observations, or rank-3 frames in front of a cnn (the model checks the cnn); the arena keeps the env's dtype
+    # (experience.py:376): uint8 frames stay bytes and are scaled by 1/255 where the first conv and the normaliser read them
+    is_dict = type(observation_space).__name__ == 'Dict'
+    if is_dict or len(observation_space.shape) != 1 and ('cnn' not in network_params or len(observation_space.shape) != 3):
+        raise NotImplementedError('only flat Box observations')
+    obs_shape = observation_space.shape
+    obs_dtype = torch.uint8 if len(obs_shape) == 3 and np.dtype(observation_space.dtype) == np.uint8 else torch.float32
+    kind = type(action_space).__name__          # a2c_common.py:1211-1224
+    if kind == 'Discrete':
+        head_sizes, actions_num, is_multi_discrete = None, int(action_space.n), False
+    elif kind == 'Tuple':
+        head_sizes = [int(a.n) for a in action_space]
+        actions_num, is_multi_discrete = sum(head_sizes), True      # width of the concatenated logits
+        if len(head_sizes) > 8:
+            raise NotImplementedError('more than 8 heads in a multi-discrete space')
+    else:
+        raise ValueError(f'Unsupported action space type for DiscreteA2CBase: {type(action_space)}')
+    if max(head_sizes or [actions_num]) > 64:
+        raise NotImplementedError('more than 64 actions in one discrete head')
+    # True: every conv and linear layer on the bf16 tensor cores (conv_tc.cu, gemm_tc.cu); False or absent: the fp32 kernels
+    mixed_precision = bool(config.get('mixed_precision') or False)
+    return obs_shape, obs_dtype, head_sizes, actions_num, is_multi_discrete, mixed_precision
+
+
 class DiscreteModel(FlatParamModel):
     """Flat fp32 parameter arena of A2CBuilder.Network for a discrete space.  Arena order: [actor conv trunk, [critic conv trunk]],
     actor MLP, [critic MLP], fused head W_head [1 + K, Hl] (row 0 = value, rows 1.. = logits) and b_head [1 + K]; ``_param_views``
@@ -254,30 +281,10 @@ class DiscreteA2CAgent(A2CBase):
             raise ValueError("PPO next_step autoreset masking does not support multi-agent envs; "
                              "wrap the env with a same_step autoreset adapter instead")
         self.observation_space = self.env_info['observation_space']
-        # flat Box observations, or rank-3 frames in front of a cnn (the model checks the cnn); the arena keeps the env's dtype
-        # (experience.py:376): uint8 frames stay bytes and are scaled by 1/255 where the first conv and the normaliser read them
-        is_dict = type(self.observation_space).__name__ == 'Dict'
-        if is_dict or len(self.observation_space.shape) != 1 and ('cnn' not in self.network_params or len(self.observation_space.shape) != 3):
-            raise NotImplementedError('only flat Box observations')
-        self.obs_shape = self.observation_space.shape
-        self.obs_dtype = torch.uint8 if len(self.obs_shape) == 3 and np.dtype(self.observation_space.dtype) == np.uint8 else torch.float32
-        action_space = self.env_info['action_space']
-        kind = type(action_space).__name__          # a2c_common.py:1211-1224
-        if kind == 'Discrete':
-            self.head_sizes, self.actions_num, self.is_multi_discrete = None, int(action_space.n), False
-        elif kind == 'Tuple':
-            self.head_sizes = [int(a.n) for a in action_space]
-            self.actions_num, self.is_multi_discrete = sum(self.head_sizes), True      # width of the concatenated logits
-            if len(self.head_sizes) > 8:
-                raise NotImplementedError('more than 8 heads in a multi-discrete space')
-        else:
-            raise ValueError(f'Unsupported action space type for DiscreteA2CBase: {type(action_space)}')
+        (self.obs_shape, self.obs_dtype, self.head_sizes, self.actions_num, self.is_multi_discrete,
+         self.mixed_precision) = discrete_spaces(self.observation_space, self.env_info['action_space'], self.network_params, config)
         self.is_discrete = True
-        if max(self.head_sizes or [self.actions_num]) > 64:
-            raise NotImplementedError('more than 64 actions in one discrete head')
         self.use_action_masks = bool(config.get('use_action_masks', False))
-        # True: every conv and linear layer on the bf16 tensor cores (conv_tc.cu, gemm_tc.cu); False or absent: the fp32 kernels
-        self.mixed_precision = bool(config.get('mixed_precision') or False)
 
     def _make_writer(self):
         return make_summary_writer(self.summaries_dir)          # on every rank

@@ -716,6 +716,13 @@ def categorical_sample(logits, ld, K, value_raw, value_ld, action_masks, u_tape,
                                             ptr(prev_dones), ptr(valid_out), N, int(values_only), _stream()), 'categorical_sample')
 
 
+def categorical_argmax(logits, ld, K, action_masks, actions_out, N, head_sizes=None):
+    """deterministic discrete action (csrc/player.cu): per-head argmax of the allowed logits into actions_out int64 [N, n_heads]"""
+    nh, tab = _head_table(head_sizes)
+    check(lib.b200rl_categorical_argmax_f32(ptr(logits), ld, K, nh, None if tab is None else ctypes.addressof(tab), ptr(action_masks),
+                                            ptr(actions_out), N, _stream()), 'categorical_argmax')
+
+
 def categorical_loss(logits, ld, K, values, value_ld, actions, action_masks, old_values_n, returns_n, old_neglogp, advs_n, mask,
                      rows_per_chunk, chunk_stride, M, cfg, inv_count, d_logits, d_ld, d_value, dv_ld, partials, head_sizes=None):
     nb = ctypes.c_int(0)

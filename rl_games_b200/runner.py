@@ -79,6 +79,15 @@ def register(runner):
     return runner
 
 
+def register_players(runner):
+    """Put the CUDA players (rl_games_b200.players) behind the reference's algo names in any runner with a `player_factory`
+    ObjectFactory -- the reference's own `rl_games.torch_runner.Runner` (torch_runner.py:122-126) or this module's mirror"""
+    from .players import player_builders
+    for name, builder in player_builders():
+        runner.player_factory.register_builder(name, builder)
+    return runner
+
+
 def register_sac(runner):
     """Put the B200 SAC agent behind the reference's algo name `sac` in any runner with an `algo_factory` ObjectFactory"""
     runner.algo_factory.register_builder('sac', lambda **kwargs: sac_agent(**kwargs))
@@ -90,6 +99,7 @@ class Runner:
         self.algo_factory = ObjectFactory()
         register(self)
         self.player_factory = ObjectFactory()
+        register_players(self)
         self._observer_was_injected = algo_observer is not None
         self.algo_observer = algo_observer if algo_observer else DefaultAlgoObserver()
 
@@ -157,8 +167,12 @@ class Runner:
         return agent.train()
 
     def run_play(self, args):
-        raise NotImplementedError('players (inference) are outside the B200 hot path; checkpoints written by this '
-                                  'trainer load into the reference players unchanged')
+        """torch_runner.py:323-334"""
+        print('Started to play')
+        player = self.create_player()
+        _restore(player, args)
+        _override_sigma(player, args)
+        player.run()
 
     def create_player(self):
         return self.player_factory.create(self.algo_name, params=self.params)
