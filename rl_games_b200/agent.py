@@ -49,36 +49,135 @@ def rescale_actions(low, high, action):
     return action * d + m
 
 
-def rollout_precision(model, actions_num, config):
-    """(fused_ok, use_tc, gemm_tc, rollout_fp32) of a continuous policy: the kernels the rollout's policy forward runs on, resolved from
-    `mixed_precision` and `b200_rollout_fp32`; the agent and the player both take them from here"""
-    # wgmma kernels: three hidden layers that fit the compiled tile widths (u1 <= 256, u2 <= 128, u3 <= 64; narrower layers are
-    # zero-padded), elu / relu / tanh, obs <= 256 (wide observations, 64 < obs <= 256: layer 1 runs in kernels of its own,
-    # l1_fwd_tc / l1_wgrad_tc), <= 15 actions; anything else runs on the fp32 kernels
-    tc_ok = model.activation in ('elu', 'relu', 'tanh') and ops.tc_supported(model.D, model.units, actions_num, True)
-    # (a fixed sigma other than the plain log-std -- a floor, bounds, 'softplus' / 'linear' -- is applied outside the kernels on the
-    #  log-std vector they read; the fused kernels take the raw parameter from the packed arena, so such policies run layer by layer.
-    #  Separate actor / critic trunks need their gradient mask applied between the split reduction and the optimiser, which the fused
-    #  tail does in one launch: layer by layer as well.  A state-dependent sigma head runs on the fp32 or the layer-wise tensor-core
-    #  kernels: the fused kernels have 16 head rows)
-    fused_ok = tc_ok and not model.is_rnn() and not getattr(model, 'sigma_transform', False) and \
-        getattr(model, 'fixed_sigma', True) and not getattr(model, 'separate', False)
-    # None (key absent) = the reference's 'auto' (a2c_common.py:427-429): the wgmma path where this build has kernels for the geometry
-    mixed_precision = config.get('mixed_precision', None)
-    if mixed_precision is None:
-        mixed_precision = fused_ok
-    # mixed_precision: True -> the fused wgmma MLP kernels where they have the geometry (use_tc), else the SAME host composition as the
-    # fp32 path with every GEMM on the tensor cores (gemm_tc: bf16 operands, fp32 accumulate -- gemm_tc.cu): LSTM policies (gate GEMMs,
-    # BPTT), MLPs wider / deeper than the fused tiles.  The reference's autocast covers nn.LSTM and nn.Linear alike (a2c_continuous.py:173).
-    use_tc = bool(mixed_precision) and fused_ok
-    gemm_tc = bool(mixed_precision) and not fused_ok
-    # Rollout precision.  The reference evaluates the policy during the rollout OUTSIDE autocast (a2c_common.py:581-600: fp32 / TF32)
-    # and only calc_gradients under bf16 autocast (a2c_continuous.py:173).  Default here: the rollout uses the same bf16 wgmma
-    # kernels as the update, so old_neglogp / old mu come from the SAME arithmetic the first mini-epoch re-evaluates (ratio == 1 at
-    # the first minibatch, which the reference's mix does not give).  b200_rollout_fp32: True restores the reference's split: fp32
-    # CUDA-core kernels for get_action_values / get_values, bf16 tensor cores for the update.
-    rollout_fp32 = use_tc and bool(config.get('b200_rollout_fp32', False))
-    return fused_ok, use_tc, gemm_tc, rollout_fp32
+class ContinuousPolicy:
+    """The rollout forward of a continuous policy, shared by the trainer (A2CAgent) and the player (players.PpoPlayerContinuous): the
+    kernels it runs on, the step buffers it reads and writes, and one step of it.  The host class provides ``model``, ``actions_num``,
+    ``normalize_value``, ``clip_actions``, ``actions_low`` / ``actions_high``, ``rng_seed``, ``rng_epoch``, ``num_rows``,
+    ``mask_autoreset_rows`` and ``is_rnn``."""
+
+    def _init_policy(self, config):
+        """the kernels the policy runs on, resolved from `mixed_precision` and `b200_rollout_fp32`; returns whether the fused wgmma
+        kernels have the geometry"""
+        m = self.model
+        # wgmma kernels: three hidden layers that fit the compiled tile widths (u1 <= 256, u2 <= 128, u3 <= 64; narrower layers are
+        # zero-padded), elu / relu / tanh, obs <= 256 (wide observations, 64 < obs <= 256: layer 1 runs in kernels of its own,
+        # l1_fwd_tc / l1_wgrad_tc), <= 15 actions; anything else runs on the fp32 kernels
+        tc_ok = m.activation in ('elu', 'relu', 'tanh') and ops.tc_supported(m.D, m.units, self.actions_num, True)
+        # (a fixed sigma other than the plain log-std -- a floor, bounds, 'softplus' / 'linear' -- is applied outside the kernels on the
+        #  log-std vector they read; the fused kernels take the raw parameter from the packed arena, so such policies run layer by layer.
+        #  Separate actor / critic trunks need their gradient mask applied between the split reduction and the optimiser, which the fused
+        #  tail does in one launch: layer by layer as well.  A state-dependent sigma head runs on the fp32 or the layer-wise tensor-core
+        #  kernels: the fused kernels have 16 head rows)
+        fused_ok = tc_ok and not m.is_rnn() and not getattr(m, 'sigma_transform', False) and \
+            getattr(m, 'fixed_sigma', True) and not getattr(m, 'separate', False)
+        # None (key absent) = the reference's 'auto' (a2c_common.py:427-429): the wgmma path where this build has kernels for the geometry
+        mixed_precision = config.get('mixed_precision', None)
+        if mixed_precision is None:
+            mixed_precision = fused_ok
+        # mixed_precision: True -> the fused wgmma MLP kernels where they have the geometry (use_tc), else the SAME host composition as the
+        # fp32 path with every GEMM on the tensor cores (gemm_tc: bf16 operands, fp32 accumulate -- gemm_tc.cu): LSTM policies (gate GEMMs,
+        # BPTT), MLPs wider / deeper than the fused tiles.  The reference's autocast covers nn.LSTM and nn.Linear alike (a2c_continuous.py:173).
+        self.use_tc = bool(mixed_precision) and fused_ok
+        self.gemm_tc = bool(mixed_precision) and not fused_ok
+        # Rollout precision.  The reference evaluates the policy during the rollout OUTSIDE autocast (a2c_common.py:581-600: fp32 / TF32)
+        # and only calc_gradients under bf16 autocast (a2c_continuous.py:173).  Default here: the rollout uses the same bf16 wgmma
+        # kernels as the update, so old_neglogp / old mu come from the SAME arithmetic the first mini-epoch re-evaluates (ratio == 1 at
+        # the first minibatch, which the reference's mix does not give).  b200_rollout_fp32: True restores the reference's split: fp32
+        # CUDA-core kernels for get_action_values / get_values, bf16 tensor cores for the update.
+        self.rollout_fp32 = self.use_tc and bool(config.get('b200_rollout_fp32', False))
+        self.tc_wide = self.use_tc and ops.tc_kind(m.D, m.units, self.actions_num) == 2
+        self.obs_norm = _RunningStats.f32_pair(m.running_mean_std)
+        # with an LSTM in front the MLP input is h (dense, not normalised)
+        self.mlp_norm = (None, None) if (self.is_rnn and m.rnn_before_mlp) else self.obs_norm
+        self.wpack = self.wbf = None        # the weights' bf16 copies, allocated with the step buffers
+        return fused_ok
+
+    def _alloc_policy(self, H, N, l1_scratch=None):
+        """what a rollout step reads and writes, zero-initialised: H steps of N rows of outputs (the arena of a trainer, one step of a
+        player), the env actions, the done flags and autoreset masks, and the scratch of the forward.  l1_scratch: the buffer the wide-
+        observation rollout parks its layer-1 tiles in between its two launches (a trainer lends its training activation tiles).
+        With the step buffers come the bf16 copies of the weights the tensor-core kernels read, which _repack fills."""
+        m, A, dev = self.model, self.actions_num, self.model.device
+        f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)   # noqa: E731
+        u8 = lambda *s: torch.zeros(*s, dtype=torch.uint8, device=dev)    # noqa: E731
+        self.actions, self.mus, self.sigmas = f(H, N, A), f(H, N, A), f(H, N, A)
+        self.neglogpacs, self.values = f(H, N), f(H, N)
+        self.dones_buf = u8(H, N)
+        self.valid = torch.ones(H, N, dtype=torch.float32, device=dev) if self.mask_autoreset_rows else None
+        self.env_actions = f(N, A)
+        self.dones = torch.ones(N, dtype=torch.uint8, device=dev)
+        self.prev_dones = f(N) if self.mask_autoreset_rows else None
+        self.ra = [f(N, u) for u in m.units] if (self.rollout_fp32 or not self.use_tc) else []
+        if self.use_tc:
+            self.wpack = u8(ops.tc_pack_bytes(m.D, m.units, A))
+        if self.gemm_tc:
+            self.wbf = torch.empty(m.num_params, dtype=torch.bfloat16, device=dev)     # bf16 twin of the parameter arena (weight operands)
+        # the layer-wise GEMMs: MLP (fp32 path, layer-wise tensor-core path, fp32 rollout of the fused path), LSTM gates, head gradient
+        self.kernels = layerwise.Kernels(tc=self.gemm_tc, bf16_arena=(m.flat, self.wbf) if self.gemm_tc else None)
+        if self.tc_wide and l1_scratch is None:
+            l1_scratch = u8((N + 127) // 128 * ops.tc_tile_bytes(m.D, m.units, A)[0])
+        self.tc_l1_scratch = l1_scratch if self.tc_wide else None
+        if self.is_rnn:
+            Hd = m.rnn_units
+            self.rnn_h, self.rnn_c = f(N, Hd), f(N, Hd)                       # current states (a2c_common.py:652-655)
+            self.r_gates, self.r_tmp_h, self.r_tmp_c = f(N, 4 * Hd), f(N, Hd), f(N, Hd)
+            self.r_y = f(N, Hd) if m.rnn_layer_norm else None                # LayerNorm(h): the rollout's normalised output
+
+    def _repack(self):
+        """bf16 operand copies of the weights for the tensor-core kernels (after every optimiser step / weight load)."""
+        m = self.model
+        if self.wpack is not None:
+            ops.tc_pack_weights(m.W[0], m.W[1], m.W[2], m.W_head, m.D, m.units, self.actions_num, self.wpack)
+        if self.wbf is not None:
+            ops.cast_bf16(m.flat, self.wbf)
+
+    def _trunk(self, x, acts, M, rows_per_chunk=None, chunk_stride=0):
+        layerwise.forward(self.kernels, self.model.mlp, x, acts, M, self.model.mlp_in, rows_per_chunk, chunk_stride, self.mlp_norm)
+
+    def _lstm_step(self, obs, h_in, c_in, h_out, c_out):
+        """one LSTM step for all N envs (seq_length 1, models.py -> network_builder.py:452-492 -> recurrent.py): returns h_out, or its
+        LayerNorm (in self.r_y) with rnn.layer_norm"""
+        m, N = self.model, self.num_rows
+        nm, ns = self.obs_norm if m.rnn_before_mlp else (None, None)      # after the MLP the LSTM reads the trunk output
+        self.kernels.fwd(obs, m.W_ih, m.b_ih, self.r_gates, 0, x_ld=m.rnn_in, norm_mean=nm, norm_std=ns, M=N)
+        self.kernels.fwd(h_in, m.W_hh, m.b_hh, self.r_gates, 0, M=N, accumulate=True)
+        if m.rnn_layer_norm:     # the trunk / heads read LayerNorm(h); h_out / c_out stay the raw carried states
+            ops.lstm_cell_ln_fwd(self.r_gates, c_in, c_out, h_out, m.ln_w, m.ln_b, N, m.rnn_units, y_out=self.r_y)
+            return self.r_y
+        ops.lstm_cell_fwd(self.r_gates, c_in, c_out, h_out, N, m.rnn_units)
+        return h_out
+
+    def _policy_step(self, obs, t, noise=None, values_only=False):
+        """the policy on N rows: action, mu, sigma, neglogp and value into step t of the output rows, the env actions, the done flags;
+        values_only: the value alone, into last_values, without advancing the recurrent states (get_values, a2c_common.py:603-626)"""
+        m, N, A = self.model, self.num_rows, self.actions_num
+        vm = m.value_mean_std
+        if values_only:
+            out = (None, 0, None, 0, None, None, None, None, self.last_values, None, False, None, None, None, None, None, None)
+        else:
+            out = (noise, self.rng_seed, self.rng_epoch, t, self.actions[t], self.mus[t], self.sigmas[t], self.neglogpacs[t],
+                   self.values[t], self.env_actions, self.clip_actions, self.actions_low, self.actions_high, self.dones,
+                   self.dones_buf[t], self.prev_dones, None if self.valid is None else self.valid[t])
+        if self.use_tc and not self.rollout_fp32:
+            nm, ns = self.obs_norm
+            ops.tc_mlp_fwd_rollout(obs, m.D, nm, ns, self.wpack, m.b, m.b_head, m.sigma, m.units, N, A, vm.running_mean,
+                                   vm.running_var, self.normalize_value, *out, values_only=values_only, l1_scratch=self.tc_l1_scratch,
+                                   activation=m.act_id)
+            return
+        if self.is_rnn:
+            h_out, c_out = (self.r_tmp_h, self.r_tmp_c) if values_only else (self.rnn_h, self.rnn_c)
+        if self.is_rnn and m.rnn_before_mlp:
+            obs = self._lstm_step(obs, self.rnn_h, self.rnn_c, h_out, c_out)
+        self._trunk(obs, self.ra, N)
+        a_last = self.ra[-1]
+        if self.is_rnn and not m.rnn_before_mlp:
+            a_last = self._lstm_step(a_last, self.rnn_h, self.rnn_c, h_out, c_out)
+        if not m.fixed_sigma:
+            ops.policy_head_sample_sd(a_last, m.W_head, m.b_head, m.sigma_cfg, vm.running_mean, vm.running_var, self.normalize_value,
+                                      *out, N, A, values_only=values_only)
+        else:
+            ops.policy_head_sample(a_last, m.W_head, m.b_head, m.sigma if values_only else m.logstd_in, vm.running_mean,
+                                   vm.running_var, self.normalize_value, *out, N, A, values_only=values_only)
 
 
 class _Dataset:
@@ -108,7 +207,7 @@ class _Dataset:
         return d
 
 
-class A2CAgent(A2CBase):
+class A2CAgent(ContinuousPolicy, A2CBase):
     def __init__(self, base_name, params):
         config = params['config']
         # options of A2CBase that change what a run does and are not built here: refuse, never ignore
@@ -140,7 +239,7 @@ class A2CAgent(A2CBase):
         # hardware supports it, a2c_common.py:427-429) and resolves to the wgmma path where this build has kernels for the
         # geometry, else to fp32 (a HIGHER precision than the reference's default), saying so once.
         self.is_rnn = self.model.is_rnn()
-        fused_ok, self.use_tc, self.gemm_tc, self.rollout_fp32 = rollout_precision(self.model, self.actions_num, config)
+        fused_ok = self._init_policy(config)
         if self.mixed_precision is None:
             self.mixed_precision = fused_ok
             if not self.mixed_precision and self.global_rank == 0:
@@ -154,10 +253,6 @@ class A2CAgent(A2CBase):
                 raise ValueError(f"Horizon length ({self.horizon_length}) must be divisible by sequence length ({self.seq_length})")
             if not self.zero_rnn_on_done:
                 raise NotImplementedError('zero_rnn_on_done: False is not on the B200 hot path')
-        self.obs_norm = _RunningStats.f32_pair(self.model.running_mean_std)
-        # with an LSTM in front the MLP input is h (dense, not normalised)
-        self.mlp_norm = (None, None) if (self.is_rnn and self.model.rnn_before_mlp) else self.obs_norm
-        self.tc_wide = self.use_tc and ops.tc_kind(self.model.D, self.model.units, self.actions_num) == 2
         if self.use_tc and config.get('b200_pipelined_wgrad', False) and (self.tc_wide or list(self.model.units) != [256, 128, 64]):
             raise NotImplementedError('b200_pipelined_wgrad is an option of the native resident-weights geometry (obs <= 64, MLP [256,128,64])')
         self.dataset = _Dataset(self)
@@ -232,45 +327,36 @@ class A2CAgent(A2CBase):
         H, N, D, A = self.horizon_length, self.num_rows, self.obs_shape[0], self.actions_num
         dev = self.device_t
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)   # noqa: E731
+        m, mb = self.model, self.minibatch_size
+        u8 = lambda n: torch.zeros(n, dtype=torch.uint8, device=dev)   # noqa: E731
+        if self.use_tc:
+            tb = ops.tc_tile_bytes(m.D, m.units, A)
+            nt = (mb + 127) // 128
+            # wide observations: the rollout's layer-1 kernel parks its a1 tiles (N rows) in the act1 buffer between the two launches
+            nt1 = max(nt, (N + 127) // 128) if self.tc_wide else nt
+            self.tc_act = [u8(nt1 * tb[0]), u8(nt * tb[1]), u8(nt * tb[2])]
+        self._alloc_policy(H, N, l1_scratch=self.tc_act[0] if self.tc_wide else None)
         self.obses = f(H, N, D)
-        self.actions, self.mus, self.sigmas = f(H, N, A), f(H, N, A), f(H, N, A)
-        self.neglogpacs, self.values, self.rewards = f(H, N), f(H, N), f(H, N)
-        self.dones_buf = torch.zeros(H, N, dtype=torch.uint8, device=dev)
-        self.valid = torch.ones(H, N, dtype=torch.float32, device=dev) if self.mask_autoreset_rows else None
+        self.rewards = f(H, N)
         self.advs, self.returns = f(H, N), f(H, N)
         self.old_values_n, self.returns_n, self.advs_n = f(H, N), f(H, N), f(H, N)
         self.last_values = f(N)
-        self.env_actions = f(N, A)
         # rl_games names (experience.py:372-398) -> arena views, for observers / tests
         self.tensor_dict = {'obses': self.obses, 'rewards': self.rewards.unsqueeze(2), 'values': self.values.unsqueeze(2),
                             'neglogpacs': self.neglogpacs, 'dones': self.dones_buf, 'actions': self.actions,
                             'mus': self.mus, 'sigmas': self.sigmas}
         # episode bookkeeping (a2c_common.py:662-666)
         self.ep_state = f(3, N)
-        self.dones = torch.ones(N, dtype=torch.uint8, device=dev)
-        self.prev_dones = f(N) if self.mask_autoreset_rows else None
         self.meter = torch.zeros(8, dtype=torch.float64, device=dev)
         self.rng_epoch = torch.zeros(1, dtype=torch.int64, device=dev)
         # workspaces
-        m, mb = self.model, self.minibatch_size
-        if self.rollout_fp32:
-            self.ra = [f(N, u) for u in m.units]
         if not self.use_tc:
-            self.ra = [f(N, u) for u in m.units]
             self.ta = [f(mb, u) for u in m.units]
             self.dA = [f(mb, u) for u in m.units]
             self.d_head = f(mb, m.head_rows)
         ops.set_pdl(self.config.get('b200_pdl', False))     # programmatic dependent launch: off by default
         if self.use_tc:
             self.n_splits = ops.NUM_SMS      # split-partial rows: at least the fused backward kernels' grid (<= one CTA per SM)
-            tb = ops.tc_tile_bytes(m.D, m.units, A)
-            nt = (mb + 127) // 128
-            u8 = lambda n: torch.zeros(n, dtype=torch.uint8, device=dev)   # noqa: E731
-            self.wpack = u8(ops.tc_pack_bytes(m.D, m.units, A))
-            # wide observations: the rollout's layer-1 kernel parks its a1 tiles (N rows) in the act1 buffer between the two launches
-            nt1 = max(nt, (N + 127) // 128) if self.tc_wide else nt
-            self.tc_act = [u8(nt1 * tb[0]), u8(nt * tb[1]), u8(nt * tb[2])]
-            self.tc_l1_scratch = self.tc_act[0] if self.tc_wide else None
             self.tc_dhead, self.tc_delta2, self.tc_delta1 = u8(nt * tb[3]), u8(nt * tb[1]), u8(nt * tb[0])
             # normalised bf16 obs tiles: the training forward emits them, the backward's layer-1 weight-gradient MMAs TMA-load
             # them instead of re-reading and re-normalising the fp32 observations (b200_emit_xtile: False restores that); config
@@ -281,33 +367,25 @@ class A2CAgent(A2CBase):
             self.tc_offs = {k: m.layout[k][0] for k in ('W0', 'b0', 'W1', 'b1', 'W2', 'b2', 'W_head', 'b_head')}
             self.pack_table = ops.tc_pack_table(m.D, m.units, A, self.tc_offs)
             self.ta = self.dA = []
-            if not self.rollout_fp32:
-                self.ra = []
         elif self.gemm_tc:
             # layer-wise tensor-core GEMMs: a weight-gradient CTA owns a [128 x <=128] tile of dW and a row split; 16 splits keep the
             # c4 gate GEMM (16 tiles) at 256 CTAs while the split partials stay small (64 splits: 91 MB of partials per gate GEMM)
             self.n_splits = max(1, min(16, mb // 512))
-            self.wbf = torch.empty(m.num_params, dtype=torch.bfloat16, device=dev)     # bf16 twin of the parameter arena (weight operands)
         else:
             self.n_splits = layerwise.n_splits(mb)
-        # the layer-wise GEMMs: MLP (fp32 path, layer-wise tensor-core path, fp32 rollout of the fused path), LSTM gates, head gradient
-        self.kernels = layerwise.Kernels(tc=self.gemm_tc, bf16_arena=(m.flat, self.wbf) if self.gemm_tc else None)
         self.part_rows = self.n_splits * (self.seq_length if self.is_rnn else 1)
         # split-partial gradient rows; the wgmma path pads the row stride to 16 bytes so the reduction can use float4 loads
         self.part = f(self.part_rows, (m.num_params + 3) // 4 * 4 if self.use_tc else m.num_params)
         if self.is_rnn:
             Hd, T = m.rnn_units, self.seq_length
             S = mb // T
-            self.rnn_h, self.rnn_c = f(N, Hd), f(N, Hd)                       # current states (a2c_common.py:652-655)
             # train-time reset flags: the buffer's dones, plus "entering the first real row after a filler reset row" on next_step envs
             self.rnn_dones_buf = torch.zeros(H, N, dtype=torch.uint8, device=dev) if self.mask_autoreset_rows else None
             self.rnn_h0, self.rnn_c0 = f(H // T, N, Hd), f(H // T, N, Hd)     # mb_rnn_states (:656-660), [num_seqs_per_env, N, hid]
-            self.r_gates, self.r_tmp_h, self.r_tmp_c = f(N, 4 * Hd), f(N, Hd), f(N, Hd)
             self.t_gates, self.t_hin, self.t_cin, self.t_c = f(T, S, 4 * Hd), f(T, S, Hd), f(T, S, Hd), f(T, S, Hd)
             self.t_hdense, self.t_hmlp, self.t_dHmlp = f(S, Hd), f(mb, Hd), f(mb, Hd)
             self.t_dgates, self.t_dhin, self.t_dcin = f(S, 4 * Hd), f(S, Hd), f(2, S, Hd)
-            if m.rnn_layer_norm:     # LayerNorm(h): the rollout's normalised output, the window's per-step row statistics for BPTT
-                self.r_y = f(N, Hd)
+            if m.rnn_layer_norm:     # the window's per-step row statistics of LayerNorm(h) for BPTT
                 self.t_mean, self.t_rstd = f(T, S), f(T, S)
         self.gae_partials = torch.zeros((N + 63) // 64, 8, dtype=torch.float64, device=dev)
         self.loss_partials = torch.zeros(max((mb + 127) // 128, ops.NUM_SMS), ops.loss_partial_stride(), dtype=torch.float64, device=dev)
@@ -541,87 +619,9 @@ class A2CAgent(A2CBase):
         return obs_t, rew, dn, infos
 
     # =============================================================================== policy forward
-    def _trunk(self, x, acts, M, rows_per_chunk=None, chunk_stride=0):
-        layerwise.forward(self.kernels, self.model.mlp, x, acts, M, self.model.mlp_in, rows_per_chunk, chunk_stride, self.mlp_norm)
-
-    def _repack(self):
-        """bf16 operand copy of the weights for the wgmma kernels (after every optimiser step / weight load)."""
-        if self.use_tc and self._tensors_ready:
-            m = self.model
-            ops.tc_pack_weights(m.W[0], m.W[1], m.W[2], m.W_head, m.D, m.units, self.actions_num, self.wpack)
-        if getattr(self, 'gemm_tc', False) and self._tensors_ready:
-            ops.cast_bf16(self.model.flat, self.wbf)
-
-    def _lstm_step(self, obs, h_in, c_in, h_out, c_out):
-        """one LSTM step for all N envs (seq_length 1, models.py -> network_builder.py:452-492 -> recurrent.py): returns h_out, or its
-        LayerNorm (in self.r_y) with rnn.layer_norm"""
-        m, N = self.model, self.num_rows
-        nm, ns = self.obs_norm if m.rnn_before_mlp else (None, None)      # after the MLP the LSTM reads the trunk output
-        self.kernels.fwd(obs, m.W_ih, m.b_ih, self.r_gates, 0, x_ld=m.rnn_in, norm_mean=nm, norm_std=ns, M=N)
-        self.kernels.fwd(h_in, m.W_hh, m.b_hh, self.r_gates, 0, M=N, accumulate=True)
-        if m.rnn_layer_norm:     # the trunk / heads read LayerNorm(h); h_out / c_out stay the raw carried states
-            ops.lstm_cell_ln_fwd(self.r_gates, c_in, c_out, h_out, m.ln_w, m.ln_b, N, m.rnn_units, y_out=self.r_y)
-            return self.r_y
-        ops.lstm_cell_fwd(self.r_gates, c_in, c_out, h_out, N, m.rnn_units)
-        return h_out
-
-    def _policy_step(self, obs, t, noise=None):
-        m, N, A = self.model, self.num_rows, self.actions_num
-        if self.use_tc and not self.rollout_fp32:
-            nm, ns = self.obs_norm
-            ops.tc_mlp_fwd_rollout(obs, m.D, nm, ns, self.wpack, m.b, m.b_head, m.sigma, m.units, N, A,
-                                   m.value_mean_std.running_mean, m.value_mean_std.running_var, self.normalize_value, noise,
-                                   self.rng_seed, self.rng_epoch, t, self.actions[t], self.mus[t], self.sigmas[t],
-                                   self.neglogpacs[t], self.values[t], self.env_actions, self.clip_actions, self.actions_low,
-                                   self.actions_high, self.dones, self.dones_buf[t], self.prev_dones,
-                                   None if self.valid is None else self.valid[t], l1_scratch=self.tc_l1_scratch, activation=m.act_id)
-            return
-        if self.is_rnn and m.rnn_before_mlp:
-            obs = self._lstm_step(obs, self.rnn_h, self.rnn_c, self.rnn_h, self.rnn_c)
-        self._trunk(obs, self.ra, N)
-        a_last = self.ra[-1]
-        if self.is_rnn and not m.rnn_before_mlp:
-            a_last = self._lstm_step(a_last, self.rnn_h, self.rnn_c, self.rnn_h, self.rnn_c)
-        if not m.fixed_sigma:
-            ops.policy_head_sample_sd(a_last, m.W_head, m.b_head, m.sigma_cfg, m.value_mean_std.running_mean,
-                                      m.value_mean_std.running_var, self.normalize_value, noise, self.rng_seed, self.rng_epoch, t,
-                                      self.actions[t], self.mus[t], self.sigmas[t], self.neglogpacs[t], self.values[t],
-                                      self.env_actions, self.clip_actions, self.actions_low, self.actions_high,
-                                      self.dones, self.dones_buf[t], self.prev_dones, None if self.valid is None else self.valid[t],
-                                      N, A)
-            return
-        ops.policy_head_sample(a_last, m.W_head, m.b_head, m.logstd_in, m.value_mean_std.running_mean,
-                               m.value_mean_std.running_var, self.normalize_value, noise, self.rng_seed, self.rng_epoch, t,
-                               self.actions[t], self.mus[t], self.sigmas[t], self.neglogpacs[t], self.values[t],
-                               self.env_actions, self.clip_actions, self.actions_low, self.actions_high,
-                               self.dones, self.dones_buf[t], self.prev_dones, None if self.valid is None else self.valid[t],
-                               N, A)
-
     def get_values(self, obs):
         """a2c_common.py:603-626"""
-        o = obs['obs'] if isinstance(obs, dict) else obs
-        m, N, A = self.model, self.num_rows, self.actions_num
-        if self.use_tc and not self.rollout_fp32:
-            nm, ns = self.obs_norm
-            ops.tc_mlp_fwd_rollout(o, m.D, nm, ns, self.wpack, m.b, m.b_head, m.sigma, m.units, N, A,
-                                   m.value_mean_std.running_mean, m.value_mean_std.running_var, self.normalize_value, None, 0, None,
-                                   0, None, None, None, None, self.last_values, None, False, None, None, None, None, None, None,
-                                   values_only=True, l1_scratch=self.tc_l1_scratch, activation=m.act_id)
-            return self.last_values.unsqueeze(1)
-        if self.is_rnn and m.rnn_before_mlp:     # get_values does not advance the agent's rnn states (a2c_common.py:603-626)
-            o = self._lstm_step(o, self.rnn_h, self.rnn_c, self.r_tmp_h, self.r_tmp_c)
-        self._trunk(o, self.ra, N)
-        a_last = self.ra[-1]
-        if self.is_rnn and not m.rnn_before_mlp:
-            a_last = self._lstm_step(a_last, self.rnn_h, self.rnn_c, self.r_tmp_h, self.r_tmp_c)
-        if not m.fixed_sigma:
-            ops.policy_head_sample_sd(a_last, m.W_head, m.b_head, m.sigma_cfg, m.value_mean_std.running_mean,
-                                      m.value_mean_std.running_var, self.normalize_value, None, 0, None, 0, None, None, None, None,
-                                      self.last_values, None, False, None, None, None, None, None, None, N, A, values_only=True)
-            return self.last_values.unsqueeze(1)
-        ops.policy_head_sample(a_last, m.W_head, m.b_head, m.sigma, m.value_mean_std.running_mean,
-                               m.value_mean_std.running_var, self.normalize_value, None, 0, None, 0, None, None, None, None,
-                               self.last_values, None, False, None, None, None, None, None, None, N, A, values_only=True)
+        self._policy_step(obs['obs'] if isinstance(obs, dict) else obs, 0, values_only=True)
         return self.last_values.unsqueeze(1)
 
     def get_action_values(self, obs, noise=None):

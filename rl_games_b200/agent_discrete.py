@@ -242,7 +242,76 @@ class _ConvTrunk:
         self.out_size = C * H * W
 
 
-class DiscreteA2CAgent(A2CBase):
+class DiscretePolicy:
+    """The forward of a discrete policy, shared by the trainer (DiscreteA2CAgent) and the player (players.PpoPlayerDiscrete): the
+    precision its conv and linear layers run on, its activation buffers and the conv + MLP forward.  The host class provides ``model``,
+    ``actions_num`` and ``mixed_precision``."""
+    wbf = None
+
+    def _init_policy(self):
+        """every conv and linear layer runs on one precision: fp32 CUDA cores, or bf16 tensor cores with the weights read from ``wbf``, a
+        bf16 twin of the parameter arena (the categorical head kernels stay fp32 either way)"""
+        m = self.model
+        self.obs_norm = _RunningStats.f32_pair(m.running_mean_std)
+        if self.mixed_precision:
+            self.wbf = torch.empty(m.num_params, dtype=torch.bfloat16, device=m.device)
+            self.kernels = layerwise.Kernels(tc=True, bf16_arena=(m.flat, self.wbf))
+        else:
+            self.kernels = layerwise.Kernels()
+
+    def _repack(self):
+        """the bf16 twin follows the fp32 arena: after every optimiser step, weight load and multi-GPU weight broadcast"""
+        if self.wbf is not None:
+            ops.cast_bf16(self.model.flat, self.wbf)
+
+    def _alloc_rows(self, M):
+        """(actor activations, critic activations, head output, actor conv activations, critic conv activations) for M rows: the MLP
+        activations' last entry is the MLP's output layer, [value | logits] (shared trunk) or the logits / the value (separate trunks);
+        the head output is its (logits, ld, value, value ld); the conv activations are NCHW rows of each conv trunk"""
+        m, K = self.model, self.actions_num
+        f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=m.device)   # noqa: E731
+        acts_a = [f(M, u) for u in m.units] + [f(M, K if m.separate else 1 + K)]
+        if m.separate:
+            acts_c = [f(M, u) for u in m.units] + [f(M, 1)]
+            out = (acts_a[-1], K, acts_c[-1], 1)
+        else:
+            acts_c, out = None, (acts_a[-1][:, 1:], K + 1, acts_a[-1], K + 1)
+        conv = lambda: [f(M, shp[0], *self._conv_out(g, shp)) for shp, g in m.cnn.layers]   # noqa: E731
+        return acts_a, acts_c, out, conv() if m.cnn else None, conv() if m.cnn and m.separate else None
+
+    @staticmethod
+    def _conv_out(g, shp):
+        C, H, W, st, pad = g
+        return (H + 2 * pad - shp[2]) // st + 1, (W + 2 * pad - shp[3]) // st + 1
+
+    def _conv_forward(self, layers, x, acts, M, rows_per_chunk, chunk_stride):
+        """acts[l] = act(conv_l(in_l)): in_0 = the observation rows (arena order, normalised), in_l = acts[l - 1]"""
+        m = self.model
+        for l, lay in enumerate(layers):
+            g = m.cnn.layers[l][1]
+            if l == 0:
+                self.kernels.conv_fwd(x, lay.W, lay.b, acts[0], g, lay.act, M, nhwc=m.cnn.nhwc, rows_per_chunk=rows_per_chunk,
+                                      chunk_stride=chunk_stride, x_ld=m.D, norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
+            else:
+                self.kernels.conv_fwd(acts[l - 1], lay.W, lay.b, acts[l], g, lay.act, M)
+
+    def _forward(self, x, acts_a, acts_c, M, rows_per_chunk=None, chunk_stride=0, conv=(None, None)):
+        """the actor MLP into acts_a (its last entry: [value | logits], or the logits with separate trunks), the critic MLP into acts_c;
+        with a cnn, each MLP reads its conv trunk's output (conv = (actor conv activations, critic conv activations))"""
+        m = self.model
+        if m.cnn:
+            self._conv_forward(m.actor_conv, x, conv[0], M, rows_per_chunk, chunk_stride)
+            layerwise.forward(self.kernels, m.actor_mlp, conv[0][-1].view(M, -1), acts_a, M, m.mlp_in)
+            if m.separate:
+                self._conv_forward(m.critic_conv, x, conv[1], M, rows_per_chunk, chunk_stride)
+                layerwise.forward(self.kernels, m.critic_mlp, conv[1][-1].view(M, -1), acts_c, M, m.mlp_in)
+            return
+        layerwise.forward(self.kernels, m.actor_mlp, x, acts_a, M, m.D, rows_per_chunk, chunk_stride, self.obs_norm)
+        if m.separate:
+            layerwise.forward(self.kernels, m.critic_mlp, x, acts_c, M, m.D, rows_per_chunk, chunk_stride, self.obs_norm)
+
+
+class DiscreteA2CAgent(DiscretePolicy, A2CBase):
     # torch_ext.AverageMeter means (float32) for the reward / episode-length summaries
     episode_summary_dtype = np.float32
 
@@ -321,36 +390,21 @@ class DiscreteA2CAgent(A2CBase):
         self.prev_dones = f(N) if self.mask_autoreset_rows else None
         self.meter = torch.zeros(8, dtype=torch.float64, device=dev)
         self.rng_epoch = torch.zeros(1, dtype=torch.int64, device=dev)
-        # activations of the actor MLP (and the critic MLP when separate), rollout (r_) and training (t_), and their gradients (d_); the
-        # last entry is the MLP's output layer: [value | logits] (shared trunk) or the logits / the value (separate trunks)
-        self.r_a, self.t_a, self.d_a = ([f(M, u) for u in m.units] + [f(M, K if m.separate else 1 + K)] for M in (N, mb, mb))
-        # (logits, ld, value, value ld) of the head output (rollout, training) and of its gradient
-        if m.separate:
-            self.r_c, self.t_c, self.d_c = ([f(M, u) for u in m.units] + [f(M, 1)] for M in (N, mb, mb))
-            self.r_out, self.t_out, self.d_out = ((a[-1], K, c[-1], 1) for a, c in ((self.r_a, self.r_c), (self.t_a, self.t_c),
-                                                                                    (self.d_a, self.d_c)))
-        else:
-            self.r_c = self.t_c = self.d_c = None
-            self.r_out, self.t_out, self.d_out = ((a[-1][:, 1:], K + 1, a[-1], K + 1) for a in (self.r_a, self.t_a, self.d_a))
+        # buffers of the rollout (r_) and training (t_) forwards and of the gradients (d_; the conv ones: pre-activation)
+        self.r_a, self.r_c, self.r_out, self.r_ka, self.r_kc = self._alloc_rows(N)
+        self.t_a, self.t_c, self.t_out, self.t_ka, self.t_kc = self._alloc_rows(mb)
+        self.d_a, self.d_c, self.d_out, self.d_ka, self.d_kc = self._alloc_rows(mb)
         if self.mixed_precision:
             # tensor-core weight gradients: a CTA owns a [128 x <=128] tile of dW and a row split; the continuous agent's layer-wise
             # rule (16 splits at most) keeps enough CTAs per layer while the split partials stay small
             self.n_splits = max(1, min(16, mb // 512))
-            self.wbf = torch.empty(m.num_params, dtype=torch.bfloat16, device=dev)     # bf16 twin of the parameter arena (weight operands)
-            ops.cast_bf16(m.flat, self.wbf)
         else:
             self.n_splits = layerwise.n_splits(mb)
-            self.wbf = None
-        if m.cnn:
-            # conv activations (NCHW rows) of each trunk, rollout / training, and their gradients (pre-activation); the conv weight
-            # gradients split over the output pixels' rows, so they take more split rows than the MLP (the leading conv_params columns)
-            conv_bufs = lambda M: [f(M, shp[0], *self._conv_out(g, shp)) for shp, g in m.cnn.layers]   # noqa: E731
-            self.r_ka, self.t_ka, self.d_ka = conv_bufs(N), conv_bufs(mb), conv_bufs(mb)
-            self.r_kc, self.t_kc, self.d_kc = (conv_bufs(N), conv_bufs(mb), conv_bufs(mb)) if m.separate else (None, None, None)
-            self.conv_splits = layerwise.n_splits(mb * m.cnn.out_shape[1] * m.cnn.out_shape[2])
-        else:
-            self.r_ka = self.t_ka = self.d_ka = self.r_kc = self.t_kc = self.d_kc = None
-            self.conv_splits = 0
+        self._init_policy()
+        self._repack()
+        # the conv weight gradients split over the output pixels' rows, so they take more split rows than the MLP (the leading
+        # conv_params columns)
+        self.conv_splits = layerwise.n_splits(mb * m.cnn.out_shape[1] * m.cnn.out_shape[2]) if m.cnn else 0
         self.part = f(max(self.n_splits, self.conv_splits), m.num_params)
         self.grad = f(m.num_params)
         self.diag_exp_var = f(self.num_minibatches) if self.diag_on else None
@@ -371,10 +425,6 @@ class DiscreteA2CAgent(A2CBase):
         rs = self.rewards_shaper
         self.shaper_cfg = ops.ShaperCfg(float(rs.scale_value), float(rs.shift_value), float(rs.min_val), float(rs.max_val),
                                         float(self.gamma), int(bool(rs.log_val)), int(bool(self.value_bootstrap)))
-        self.obs_norm = _RunningStats.f32_pair(m.running_mean_std)
-        # every conv and linear layer of the rollout and the update runs on one precision: fp32 CUDA cores, or bf16 tensor cores with
-        # the weights read from the twin (the categorical head kernels stay fp32 either way)
-        self.kernels = layerwise.Kernels(tc=True, bf16_arena=(m.flat, self.wbf)) if self.mixed_precision else layerwise.Kernels()
         self._tensors_ready = True
 
     # =============================================================================== env plumbing (tensor envs on the device)
@@ -398,23 +448,7 @@ class DiscreteA2CAgent(A2CBase):
         o, rewards, dones, infos = self.vec_env.step(actions)
         return self._obs_rows(o), self._to_dev(rewards, torch.float32), self._to_dev(dones), infos
 
-    # =============================================================================== forward
-    @staticmethod
-    def _conv_out(g, shp):
-        C, H, W, st, pad = g
-        return (H + 2 * pad - shp[2]) // st + 1, (W + 2 * pad - shp[3]) // st + 1
-
-    def _conv_forward(self, layers, x, acts, M, rows_per_chunk, chunk_stride):
-        """acts[l] = act(conv_l(in_l)): in_0 = the observation rows (arena order, normalised), in_l = acts[l - 1]"""
-        m = self.model
-        for l, lay in enumerate(layers):
-            g = m.cnn.layers[l][1]
-            if l == 0:
-                self.kernels.conv_fwd(x, lay.W, lay.b, acts[0], g, lay.act, M, nhwc=m.cnn.nhwc, rows_per_chunk=rows_per_chunk,
-                                      chunk_stride=chunk_stride, x_ld=m.D, norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
-            else:
-                self.kernels.conv_fwd(acts[l - 1], lay.W, lay.b, acts[l], g, lay.act, M)
-
+    # =============================================================================== backward
     def _conv_backward(self, layers, x, acts, grads, M, rows_per_chunk, chunk_stride):
         """grads[-1] = dL/d(pre-activation of the last conv) in; weight gradients into the leading columns of `part`"""
         m, P = self.model, self.model.num_params
@@ -429,21 +463,6 @@ class DiscreteA2CAgent(A2CBase):
                 k.conv_bwd_weight(grads[l], acts[l - 1], self.part[0, lay.w_off:], self.part[0, lay.b_off:], lay.W.shape, g,
                                   self.conv_splits, M, P)
                 k.conv_bwd_data(grads[l], lay.W, acts[l - 1], grads[l - 1], g, layers[l - 1].act, M)
-
-    def _forward(self, x, acts_a, acts_c, M, rows_per_chunk=None, chunk_stride=0, conv=(None, None)):
-        """the actor MLP into acts_a (its last entry: [value | logits], or the logits with separate trunks), the critic MLP into acts_c;
-        with a cnn, each MLP reads its conv trunk's output (conv = (actor conv activations, critic conv activations))"""
-        m = self.model
-        if m.cnn:
-            self._conv_forward(m.actor_conv, x, conv[0], M, rows_per_chunk, chunk_stride)
-            layerwise.forward(self.kernels, m.actor_mlp, conv[0][-1].view(M, -1), acts_a, M, m.mlp_in)
-            if m.separate:
-                self._conv_forward(m.critic_conv, x, conv[1], M, rows_per_chunk, chunk_stride)
-                layerwise.forward(self.kernels, m.critic_mlp, conv[1][-1].view(M, -1), acts_c, M, m.mlp_in)
-            return
-        layerwise.forward(self.kernels, m.actor_mlp, x, acts_a, M, m.D, rows_per_chunk, chunk_stride, self.obs_norm)
-        if m.separate:
-            layerwise.forward(self.kernels, m.critic_mlp, x, acts_c, M, m.D, rows_per_chunk, chunk_stride, self.obs_norm)
 
     # =============================================================================== rollout
     def play_steps(self, u=None):
@@ -555,11 +574,6 @@ class DiscreteA2CAgent(A2CBase):
                       n=P)
         self._repack()
         return stats
-
-    def _repack(self):
-        """the bf16 twin follows the fp32 arena: after every optimiser step, weight load and multi-GPU weight broadcast"""
-        if getattr(self, 'wbf', None) is not None:
-            ops.cast_bf16(self.model.flat, self.wbf)
 
     def train_epoch(self, u=None):
         """DiscreteA2CBase.train_epoch (a2c_common.py:1233-1289): returns the reference's tuple."""

@@ -38,7 +38,45 @@ _KNOWN_KEYS = {
 }
 
 
-class SACAgent(CompileTolerantModel):
+class SACActor:
+    """The acting half of SAC, shared by the trainer (SACAgent) and the player (players.SACPlayer): the action box, the rollout's Philox
+    key and counter, the rollout buffers and one action step on the fp32 kernels.  The host class provides ``model``, ``A`` and ``D``."""
+
+    def _init_actor(self, params, act_space):
+        dev = self.model.device
+        self.action_low = torch.tensor(act_space.low, dtype=torch.float32).to(dev)
+        self.action_high = torch.tensor(act_space.high, dtype=torch.float32).to(dev)
+        self.action_scale = (self.action_high - self.action_low) / 2.0
+        self.action_bias = (self.action_high + self.action_low) / 2.0
+        self.act_box = (self.action_scale, self.action_bias, self.action_low, self.action_high)
+        self.seed = int(params.get('seed', 0) or 0) & 0xFFFFFFFFFFFFFFFF
+        self.roll_ctr = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.obs_norm = _RunningStats.f32_pair(self.model.running_mean_std)
+        # the passes the reference runs outside autocast -- the rollout's act(), the critic target's actor and target critics
+        # (sac_agent.py update_critic) -- run on the fp32 kernels whatever mixed_precision says
+        self.k32 = layerwise.Kernels()
+
+    def _alloc_actor(self, N):
+        f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.model.device)       # noqa: E731
+        self.roll_acts = [f(N, w) for w in self.model.units] + [f(N, 2 * self.A)]
+        self.actions = f(N, self.A)
+        self.obs_buf = f(N, self.D)
+
+    def _act(self, obs, random_exploration, tape=None):
+        """actions of the rollout rows: uniform in the box (random exploration), else the squashed Gaussian policy; tape: [N, A] uniforms
+        or normals in place of the Philox draws"""
+        m, N = self.model, self.actions.shape[0]
+        if random_exploration:
+            ops.sac_uniform_actions(self.action_low, self.action_high, tape, self.seed, self.roll_ctr, self.actions, N, self.A)
+        else:
+            layerwise.forward(self.k32, m.actor_mlp, obs, self.roll_acts, N, self.D, norm=self.obs_norm)
+            ops.sac_squash_fwd(self.roll_acts[-1], N, self.A, m.log_std_bounds, tape, self.seed, self.roll_ctr, ops.SAC_SITE_ROLLOUT,
+                               self.act_box, 0.0, dst=self.actions, dst_ld=self.A)
+        ops.bump_u64(self.roll_ctr)
+        return self.actions
+
+
+class SACAgent(SACActor, CompileTolerantModel):
     def __init__(self, base_name, params):
         self.config = config = params['config']
         self.name = base_name
@@ -122,17 +160,12 @@ class SACAgent(CompileTolerantModel):
                       tuple(config.get('alphas_betas', [0.9, 0.999])))
 
         dev = self.device_t
-        self.action_low = torch.tensor(act_space.low, dtype=torch.float32).to(dev)
-        self.action_high = torch.tensor(act_space.high, dtype=torch.float32).to(dev)
-        self.action_scale = (self.action_high - self.action_low) / 2.0
-        self.action_bias = (self.action_high + self.action_low) / 2.0
         lss = torch.log(((torch.tensor(act_space.high, dtype=torch.float32) - torch.tensor(act_space.low, dtype=torch.float32)) / 2.0)
                         .clamp_min(1e-8)).sum()
         self.log_action_scale_sum = float(lss)
-        self.act_box = (self.action_scale, self.action_bias, self.action_low, self.action_high)
 
         self.model = SACModel(self.network_params, self.D, self.A, dev, self.normalize_input, self.init_alpha)
-        self.seed = int(params.get('seed', 0) or 0) & 0xFFFFFFFFFFFFFFFF
+        self._init_actor(params, act_space)
 
         self.frame = self.epoch_num = 0
         self.last_mean_rewards = -float('inf')
@@ -174,7 +207,6 @@ class SACAgent(CompileTolerantModel):
         self.ep_state = f(2 * N)
         self.meter = torch.zeros(3, dtype=torch.float64, device=dev)
         self.rng_ctr = torch.zeros(1, dtype=torch.int64, device=dev)
-        self.roll_ctr = torch.zeros(1, dtype=torch.int64, device=dev)
         u = self.model.units
         self.x_cur, self.x_pi, self.x_next = f(B, D + A), f(B, D + A), f(B, D + A)
         self.reward_b, self.not_done_b = f(B), f(B)
@@ -190,9 +222,7 @@ class SACAgent(CompileTolerantModel):
         self.dx_in = [f(B, D + A), f(B, D + A)]
         self.eps_pi = f(B, A)
         self.logp_next, self.logp_pi = f(B), f(B)
-        self.roll_acts = [f(N, w) for w in u] + [f(N, 2 * A)]
-        self.actions = f(N, A)
-        self.obs_buf = f(N, D)
+        self._alloc_actor(N)
         self.n_splits = layerwise.n_splits(B)
         m = self.model
         self.part_a = f(self.n_splits, m.actor.n)
@@ -207,10 +237,6 @@ class SACAgent(CompileTolerantModel):
         if self.normalize_input:
             self.rms_scratch = torch.zeros(ops.NUM_SMS * 2 * D, dtype=torch.float64, device=dev)
             self.rms_counter = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.obs_norm = _RunningStats.f32_pair(self.model.running_mean_std)
-        # the passes the reference runs outside autocast -- the critic target's actor and target critics (sac_agent.py update_critic),
-        # the rollout's act() -- run on the fp32 kernels whatever mixed_precision says
-        self.k32 = layerwise.Kernels()
         self.kernels = layerwise.Kernels(tc=self.mixed_precision)
 
     def init_tensors(self):
@@ -341,17 +367,6 @@ class SACAgent(CompileTolerantModel):
         self.prev_dones.zero_()
         return obs
 
-    def _act(self, obs, random_exploration):
-        m, N = self.model, self.num_actors
-        if random_exploration:
-            ops.sac_uniform_actions(self.action_low, self.action_high, self._tape('u'), self.seed, self.roll_ctr, self.actions, N, self.A)
-        else:
-            layerwise.forward(self.k32, m.actor_mlp, obs, self.roll_acts, N, self.D, norm=self.obs_norm)
-            ops.sac_squash_fwd(self.roll_acts[-1], N, self.A, m.log_std_bounds, self._tape('noise_roll'), self.seed, self.roll_ctr,
-                               ops.SAC_SITE_ROLLOUT, self.act_box, 0.0, dst=self.actions, dst_ld=self.A)
-        ops.bump_u64(self.roll_ctr)
-        return self.actions
-
     def _store(self, obs, action, rewards, next_obs, dones, infos):
         """_store_transitions: shaped reward, terminated / truncated split, the replay write and the episode accounting, on the device"""
         shaped = self._to_dev(self.rewards_shaper(self._to_dev(rewards))).reshape(-1).contiguous()
@@ -377,7 +392,7 @@ class SACAgent(CompileTolerantModel):
         n_upd = 0
         actor_rows = []
         for _ in range(self.num_steps_per_episode):
-            action = self._act(obs, random_exploration)
+            action = self._act(obs, random_exploration, self._tape('u' if random_exploration else 'noise_roll'))
             t0 = time.perf_counter()
             # the env gets a copy: the action buffer is rewritten by the next step's sampler
             env_actions = action.clone() if self._tensor_env else action.cpu().numpy()

@@ -3,10 +3,10 @@ rl_games.algos_torch.players (PpoPlayerContinuous, PpoPlayerDiscrete, SACPlayer)
 
 Same constructor (``Player(params)``), config keys (``player: {games_num, n_game_life, deterministic, print_stats, render,
 render_sleep, balance_env_rewards, use_vecenv, env_config}``), ``run()`` loop and printed lines as the reference's players, and the same
-checkpoints (``restore(fn)``).  The policy is evaluated by the forward code of the training agents themselves -- ``A2CAgent._policy_step``
-/ ``_lstm_step`` / ``_trunk``, ``DiscreteA2CAgent._forward`` / ``_conv_forward``, ``SACAgent._act`` -- run on the player's own buffers
-(one step of N = the detected batch rows), so a policy is played in the arithmetic its rollout was trained with: the precision keys
-(``mixed_precision``, ``b200_rollout_fp32``) resolve as in the agent.  Deterministic actions are ``mu`` (a zero noise tape through the
+checkpoints (``restore(fn)``).  The policy is evaluated by the forward code the training agents run -- each player derives from its family's
+policy base, ``agent.ContinuousPolicy``, ``agent_discrete.DiscretePolicy`` or ``agent_sac.SACActor``, as the agent does -- on the
+player's own step buffers (one step of N = the detected batch rows), so a policy is played in the arithmetic its rollout was trained
+with: the precision keys (``mixed_precision``, ``b200_rollout_fp32``) resolve as in the agent.  Deterministic actions are ``mu`` (a zero noise tape through the
 Gaussian head kernels, which also apply the clamp and the env rescale), ``tanh(mu)`` rescaled and clamped for SAC (a zero noise tape
 through ``sac_squash_fwd``) and the per-head argmax of the masked logits (``categorical_argmax``).  Sampled actions come from the
 rollout's Philox streams, keyed as the agents key them (PPO: ``b200_rng_seed``, else ``seed``; SAC: ``seed``) with the player's step
@@ -23,12 +23,11 @@ import numpy as np
 import torch
 
 from . import ops
-from .agent import A2CAgent, rollout_precision
-from .agent_discrete import DiscreteA2CAgent, DiscreteModel, discrete_spaces
-from .agent_sac import SACAgent
+from .agent import ContinuousPolicy
+from .agent_discrete import DiscreteModel, DiscretePolicy, discrete_spaces
+from .agent_sac import SACActor
 from .common import configurations, create_vec_env
-from .layerwise import Kernels
-from .model import B200Model, _RunningStats, resolve_device
+from .model import B200Model, resolve_device
 from .model_sac import SACModel
 
 
@@ -384,12 +383,9 @@ class BasePlayer:
                 print('av reward:', sum_rewards / games_played * n_game_life, 'av steps:', sum_steps / games_played * n_game_life)
 
 
-class PpoPlayerContinuous(BasePlayer):
-    """algos_torch/players.py PpoPlayerContinuous on A2CAgent's rollout forward"""
-    _trunk = A2CAgent._trunk
-    _lstm_step = A2CAgent._lstm_step
-    _policy_step = A2CAgent._policy_step
-    _repack = A2CAgent._repack
+class PpoPlayerContinuous(ContinuousPolicy, BasePlayer):
+    """algos_torch/players.py PpoPlayerContinuous on the continuous policy's rollout forward"""
+    mask_autoreset_rows = False
 
     def __init__(self, params):
         super().__init__(params)
@@ -409,17 +405,8 @@ class PpoPlayerContinuous(BasePlayer):
         self.is_rnn = self.model.is_rnn()
         if self.is_rnn and not config.get('zero_rnn_on_done', True):
             raise NotImplementedError('zero_rnn_on_done: False is not on the B200 hot path')
-        _, self.use_tc, self.gemm_tc, self.rollout_fp32 = rollout_precision(self.model, self.actions_num, config)
-        self.obs_norm = _RunningStats.f32_pair(self.model.running_mean_std)
-        self.mlp_norm = (None, None) if (self.is_rnn and self.model.rnn_before_mlp) else self.obs_norm
-        self.tc_wide = self.use_tc and ops.tc_kind(self.model.D, self.model.units, self.actions_num) == 2
-        dev, m = self.device, self.model
-        self.wbf = torch.empty(m.num_params, dtype=torch.bfloat16, device=dev) if self.gemm_tc else None
-        self.kernels = Kernels(tc=self.gemm_tc, bf16_arena=(m.flat, self.wbf) if self.gemm_tc else None)
-        self.wpack = torch.zeros(ops.tc_pack_bytes(m.D, m.units, self.actions_num), dtype=torch.uint8, device=dev) if self.use_tc else None
-        self.rng_epoch = torch.zeros(1, dtype=torch.int64, device=dev)        # the Philox counter: one per player step
-        self.prev_dones, self.valid = None, None
-        self._tensors_ready = True
+        self._init_policy(config)
+        self.rng_epoch = torch.zeros(1, dtype=torch.int64, device=self.device)        # the Philox counter: one per player step
         self._weights_loaded()
 
     def _weights_loaded(self):
@@ -431,24 +418,14 @@ class PpoPlayerContinuous(BasePlayer):
         super().run()
 
     def _alloc(self, N):
-        """A2CAgent.init_tensors' rollout buffers for one step of N rows (arena time index 0)"""
-        dev, m, A = self.device, self.model, self.actions_num
-        f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)   # noqa: E731
-        self.obs_buf = f(N, m.D)
-        self.actions, self.mus, self.sigmas = f(1, N, A), f(1, N, A), f(1, N, A)
-        self.neglogpacs, self.values = f(1, N), f(1, N)
-        self.env_actions = f(N, A)
-        self.dones = torch.zeros(N, dtype=torch.uint8, device=dev)
-        self.dones_buf = torch.zeros(1, N, dtype=torch.uint8, device=dev)
-        self.zero_noise = f(N, A)
+        """the policy's step buffers for one step of N rows (output step 0), the static observation rows and the noise tapes"""
+        self._alloc_policy(1, N)
+        self._repack()
+        dev, A = self.device, self.actions_num
+        self.obs_buf = torch.zeros(N, self.model.D, dtype=torch.float32, device=dev)
+        self.zero_noise = torch.zeros(N, A, dtype=torch.float32, device=dev)
         self.noise = None           # [N, A] normal tape for sampled actions (tests); None: the Philox stream
-        self.ra = [f(N, u) for u in m.units] if (self.rollout_fp32 or not self.use_tc) else []
-        self.tc_l1_scratch = (torch.zeros((N + 127) // 128 * ops.tc_tile_bytes(m.D, m.units, A)[0], dtype=torch.uint8, device=dev)
-                              if self.tc_wide else None)
         if self.is_rnn:
-            Hd = m.rnn_units
-            self.rnn_h, self.rnn_c, self.r_gates = f(N, Hd), f(N, Hd), f(N, 4 * Hd)
-            self.r_y = f(N, Hd) if m.rnn_layer_norm else None
             self.done_dev = torch.zeros(N, dtype=torch.uint8, device=dev)
 
     def _graph_key(self, deterministic):
@@ -476,12 +453,8 @@ class PpoPlayerContinuous(BasePlayer):
         return current_action.clone()
 
 
-class PpoPlayerDiscrete(BasePlayer):
-    """algos_torch/players.py PpoPlayerDiscrete on DiscreteA2CAgent's forward"""
-    _conv_out = staticmethod(DiscreteA2CAgent._conv_out)
-    _conv_forward = DiscreteA2CAgent._conv_forward
-    _forward = DiscreteA2CAgent._forward
-    _repack = DiscreteA2CAgent._repack
+class PpoPlayerDiscrete(DiscretePolicy, BasePlayer):
+    """algos_torch/players.py PpoPlayerDiscrete on the discrete policy's forward"""
 
     def __init__(self, params):
         super().__init__(params)
@@ -495,10 +468,7 @@ class PpoPlayerDiscrete(BasePlayer):
         self.model = DiscreteModel(self.network_params, self.obs_shape, self.actions_num, self.device, self.normalize_input,
                                    self.normalize_value, head_sizes=self.head_sizes)
         self.is_rnn = False
-        m = self.model
-        self.wbf = torch.empty(m.num_params, dtype=torch.bfloat16, device=self.device) if self.mixed_precision else None
-        self.kernels = Kernels(tc=True, bf16_arena=(m.flat, self.wbf)) if self.mixed_precision else Kernels()
-        self.obs_norm = _RunningStats.f32_pair(m.running_mean_std)
+        self._init_policy()
         self.rng_epoch = torch.zeros(1, dtype=torch.int64, device=self.device)
         self._weights_loaded()
 
@@ -506,28 +476,15 @@ class PpoPlayerDiscrete(BasePlayer):
         self._repack()
 
     def _alloc(self, N):
-        """DiscreteA2CAgent.init_tensors' rollout buffers for one step of N rows"""
-        dev, m, K = self.device, self.model, self.actions_num
-        f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)   # noqa: E731
-        self.obs_buf = torch.zeros(N, m.D, dtype=self.obs_dtype, device=dev)
+        """the policy's rollout buffers for one step of N rows, the static observation and mask rows and the step's outputs"""
+        dev, K = self.device, self.actions_num
+        self.obs_buf = torch.zeros(N, self.model.D, dtype=self.obs_dtype, device=dev)
         self.mask_buf = torch.ones(N, K, dtype=torch.uint8, device=dev)
         nh = len(self.head_sizes) if self.head_sizes else 1
         self.actions_out = torch.zeros(N, nh, dtype=torch.int64, device=dev)
-        self.neglogp, self.values = f(N), f(N)
+        self.neglogp, self.values = torch.zeros(N, dtype=torch.float32, device=dev), torch.zeros(N, dtype=torch.float32, device=dev)
         self.u = None               # [n_heads, N] uniform tape for sampled actions (tests); None: the Philox stream
-        self.r_a = [f(N, u) for u in m.units] + [f(N, K if m.separate else 1 + K)]
-        if m.separate:
-            self.r_c = [f(N, u) for u in m.units] + [f(N, 1)]
-            self.r_out = (self.r_a[-1], K, self.r_c[-1], 1)
-        else:
-            self.r_c = None
-            self.r_out = (self.r_a[-1][:, 1:], K + 1, self.r_a[-1], K + 1)
-        if m.cnn:
-            conv_bufs = lambda: [f(N, shp[0], *self._conv_out(g, shp)) for shp, g in m.cnn.layers]   # noqa: E731
-            self.r_ka = conv_bufs()
-            self.r_kc = conv_bufs() if m.separate else None
-        else:
-            self.r_ka = self.r_kc = None
+        self.r_a, self.r_c, self.r_out, self.r_ka, self.r_kc = self._alloc_rows(N)
 
     def _graph_key(self, deterministic):
         return deterministic, self._masked, None if self.u is None else self.u.data_ptr()
@@ -563,9 +520,8 @@ class PpoPlayerDiscrete(BasePlayer):
         return self._act(obs, None, is_deterministic)
 
 
-class SACPlayer(BasePlayer):
-    """algos_torch/players.py SACPlayer on SACAgent's rollout forward (fp32 kernels, as the agent's rollout)"""
-    _act = SACAgent._act
+class SACPlayer(SACActor, BasePlayer):
+    """algos_torch/players.py SACPlayer on the SAC actor's rollout forward (fp32 kernels, as the agent's rollout)"""
 
     def __init__(self, params):
         super().__init__(params)
@@ -577,18 +533,9 @@ class SACPlayer(BasePlayer):
             raise NotImplementedError('SAC supports continuous Box action spaces only (discrete action spaces are not supported)')
         self.actions_num = self.A = self.action_space.shape[0]
         self.D = self.obs_shape[0]
-        dev = self.device
-        self.action_low = torch.tensor(self.action_space.low, dtype=torch.float32).to(dev)
-        self.action_high = torch.tensor(self.action_space.high, dtype=torch.float32).to(dev)
-        self.action_scale = (self.action_high - self.action_low) / 2.0
-        self.action_bias = (self.action_high + self.action_low) / 2.0
-        self.act_box = (self.action_scale, self.action_bias, self.action_low, self.action_high)
         self.normalize_input = self.config.get('normalize_input', False)
-        self.model = SACModel(self.network_params, self.D, self.A, dev, self.normalize_input, self.config.get('init_alpha', 1.0))
-        self.seed = int(params.get('seed', 0) or 0) & 0xFFFFFFFFFFFFFFFF      # the agent's rollout stream key
-        self.k32 = Kernels()
-        self.obs_norm = _RunningStats.f32_pair(self.model.running_mean_std)
-        self.roll_ctr = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.model = SACModel(self.network_params, self.D, self.A, self.device, self.normalize_input, self.config.get('init_alpha', 1.0))
+        self._init_actor(params, self.action_space)
 
     def restore(self, fn):
         checkpoint = self._load_checkpoint(fn)
@@ -601,17 +548,9 @@ class SACPlayer(BasePlayer):
         self._restore_env_state(checkpoint)
 
     def _alloc(self, N):
-        f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)   # noqa: E731
-        self.num_actors = N
-        self.obs_buf = f(N, self.D)
-        self.roll_acts = [f(N, w) for w in self.model.units] + [f(N, 2 * self.A)]
-        self.actions = f(N, self.A)
-        self.zero_noise = f(N, self.A)
+        self._alloc_actor(N)
+        self.zero_noise = torch.zeros(N, self.A, dtype=torch.float32, device=self.device)
         self.noise = None           # [N, A] normal tape for sampled actions (tests); None: the Philox stream
-        self._deterministic = True
-
-    def _tape(self, key):
-        return self.zero_noise if self._deterministic else self.noise
 
     def _graph_key(self, deterministic):
         return deterministic, None if self.noise is None else self.noise.data_ptr()
@@ -620,8 +559,7 @@ class SACPlayer(BasePlayer):
         return [self.roll_ctr]
 
     def _step_body(self, deterministic):
-        self._deterministic = deterministic
-        self._act(self.obs_buf, False)
+        self._act(self.obs_buf, False, self.zero_noise if deterministic else self.noise)
 
     def get_action(self, obs, is_deterministic=False):
         self._prepare_obs(obs)

@@ -15,6 +15,16 @@ from test_agent_gpu import DEV, TapeEnvGPU, make_agent  # noqa: E402
 pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(__file__), 'golden')
 
+@pytest.fixture(autouse=True)
+def _fp32_matmuls():
+    """the torch restatements are fp32 references: keep their GEMMs off TF32, which constructing the reference's Runner (other tests of
+    the same process do) switches on for the whole process"""
+    tf32 = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    yield
+    torch.backends.cuda.matmul.allow_tf32 = tf32
+
+
 _PARAMS = [('exp', 0.0, None), ('exp', 0.1, (-1.0, 0.4)), ('softplus', 0.2, None), ('linear', 0.0, None)]
 
 
