@@ -195,6 +195,36 @@ int b200rl_conv2d_bwd_weight_tc(const float* dY, const void* X, int x_u8, int x_
                                 int64_t x_ld, const float* norm_mean, const float* norm_std, float* dW_part, float* db_part,
                                 int64_t split_stride, int M, int C, int H, int Wd, int Cout, int KH, int KW, int stride, int pad,
                                 int n_splits, void* stream);
+/* ---------------------------------------------------------------------------------------------
+ * 1-D convolutions of a conv1d trunk (network_builder.py _build_cnn1d: nn.Conv1d + activation per layer) over frame-stacked features,
+ * the same implicit GEMMs as the conv2d functions above (the same kernels, instantiated for one spatial axis), fp32 or tensor cores.
+ * Geometry: input [C, L] (C = stacked frames, or features with the frame stack transposed), Cout filters W[Cout, C, k] (PyTorch's
+ * nn.Conv1d layout), stride and zero padding along L, output [Cout, Lo], Lo = (L + 2 pad - k) / stride + 1.  Activations and
+ * gradients are dense [M, C, L] rows; X is fp32 only (the first layer reads the arena's chunked rows, rows_per_chunk / chunk_stride /
+ * x_ld as linear_fwd, with the optional per-element normaliser of the flat [C*L] observation applied before zero padding).
+ *   conv1d_fwd:        Y = act(conv1d(norm(X)) + b)
+ *   conv1d_bwd_data:   dX = conv1d^T(dY, W) * act'(A_prev), gathered per input position (deterministic, no atomics)
+ *   conv1d_bwd_weight: dW_part[s*split_stride + ..][Cout, C*k] = sum over the output positions of row split s, db_part likewise
+ * The _tc functions run on the bf16 tensor cores with the conv2d _tc functions' precision contract, weights read from W_bf16
+ * (required, the bf16 twin of the filters) in the forward and the data gradient.  B200RL_EINVAL: a bad pointer or geometry;
+ * B200RL_EUNSUPPORTED (_tc): the conv2d _tc grid limits.
+ * ------------------------------------------------------------------------------------------- */
+int b200rl_conv1d_fwd_f32(const float* X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld, const float* norm_mean,
+                          const float* norm_std, const float* W, const float* b, float* Y, int M, int C, int L, int Cout, int k,
+                          int stride, int pad, int act, void* stream);
+int b200rl_conv1d_bwd_data_f32(const float* dY, const float* W, const float* A_prev, float* dX, int M, int C, int L, int Cout, int k,
+                               int stride, int pad, int act_prev, void* stream);
+int b200rl_conv1d_bwd_weight_f32(const float* dY, const float* X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
+                                 const float* norm_mean, const float* norm_std, float* dW_part, float* db_part, int64_t split_stride,
+                                 int M, int C, int L, int Cout, int k, int stride, int pad, int n_splits, void* stream);
+int b200rl_conv1d_fwd_tc(const float* X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld, const float* norm_mean,
+                         const float* norm_std, const void* W_bf16, const float* b, float* Y, int M, int C, int L, int Cout, int k,
+                         int stride, int pad, int act, void* stream);
+int b200rl_conv1d_bwd_data_tc(const float* dY, const void* W_bf16, const float* A_prev, float* dX, int M, int C, int L, int Cout, int k,
+                              int stride, int pad, int act_prev, void* stream);
+int b200rl_conv1d_bwd_weight_tc(const float* dY, const float* X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
+                                const float* norm_mean, const float* norm_std, float* dW_part, float* db_part, int64_t split_stride,
+                                int M, int C, int L, int Cout, int k, int stride, int pad, int n_splits, void* stream);
 /* out[i] = sum_s part[s*split_stride + i]  (deterministic, fixed order) */
 /* The same three building blocks on the tensor cores (wgmma, bf16 operands rounded while they are staged, fp32 accumulate in
  * registers, fp32 bias / activation / outputs) for ANY layer width: the mixed_precision path of LSTM gate GEMMs and of MLPs the fused

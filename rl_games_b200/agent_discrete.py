@@ -7,12 +7,13 @@ STATUS: parity-green on an H100 (``tests/test_discrete_gpu.py``) against a CPU o
 (csrc/discrete.cu) reuses the kernels of the continuous path: linear_fwd / linear_bwd_* / reduce_splits (mlp_simt.cu), gae_fused, prepare_batch, moments_update,
 mask_inv_counts (stats.cu, gae.cu), post_step (rollout.cu), adam_step (adam.cu).
 
-Image observations (``cnn: {type: conv2d}`` on a rank-3 Box) run a conv trunk (csrc/conv.cu) in front of the MLP; see DESIGN.md §4.
+Image observations (``cnn: {type: conv2d}`` on a rank-3 Box) and frame-stacked unit features (``cnn: {type: conv1d}`` on a rank-2 fp32
+Box, the smac configs) run a conv trunk (csrc/conv.cu) in front of the MLP; see DESIGN.md §4.
 Precision is read by value: ``mixed_precision: True`` runs every conv and linear layer of the rollout and the update on the bf16
 tensor cores (csrc/conv_tc.cu, csrc/gemm_tc.cu; the categorical head kernels stay fp32), with the weights read from ``wbf``, a bf16
 twin of the parameter arena refreshed after every optimiser step, weight load and weight broadcast; ``False`` or no key runs the fp32
 kernels above.
-Scope of this first edition: one GPU, eager launches (no CUDA graph), flat Box observations or conv2d frames, ``Discrete(K)`` or multi-discrete
+Scope of this first edition: one GPU, eager launches (no CUDA graph), flat Box observations, conv2d frames or conv1d frame stacks, ``Discrete(K)`` or multi-discrete
 ``Tuple(Discrete(K_j))`` action spaces (K_j <= 64, <= 8 heads), no RNN, no central value.  The scheduler steps once per MINI-EPOCH on the mean KL like the reference
 (a2c_common.py:1265-1272), which costs one host sync per mini-epoch.
 
@@ -35,11 +36,16 @@ from .model import _apply_init, check_network_params, FlatParamModel, _RunningSt
 def discrete_spaces(observation_space, action_space, network_params, config):
     """(obs_shape, obs_dtype, head_sizes, actions_num, is_multi_discrete, mixed_precision) of a discrete policy, or the refusal of its
     spaces; the agent and the player both take them from here"""
-    # flat Box observations, or rank-3 frames in front of a cnn (the model checks the cnn); the arena keeps the env's dtype
-    # (experience.py:376): uint8 frames stay bytes and are scaled by 1/255 where the first conv and the normaliser read them
+    # flat Box observations, rank-3 frames in front of a cnn (the model checks the cnn), or a rank-2 frame stack in front of a conv1d
+    # cnn; the arena keeps the env's dtype (experience.py:376): uint8 frames stay bytes and are scaled by 1/255 where the first conv and
+    # the normaliser read them
     is_dict = type(observation_space).__name__ == 'Dict'
-    if is_dict or len(observation_space.shape) != 1 and ('cnn' not in network_params or len(observation_space.shape) != 3):
+    cnn = network_params.get('cnn')
+    rank = 0 if is_dict else len(observation_space.shape)
+    if is_dict or rank != 1 and (cnn is None or rank != 3 and (rank != 2 or cnn.get('type') != 'conv1d')):
         raise NotImplementedError('only flat Box observations')
+    if rank == 2 and np.dtype(observation_space.dtype) == np.uint8:
+        raise NotImplementedError("'cnn' networks of type 'conv1d' read fp32 observations on the discrete B200 agent, got uint8")
     obs_shape = observation_space.shape
     obs_dtype = torch.uint8 if len(obs_shape) == 3 and np.dtype(observation_space.dtype) == np.uint8 else torch.float32
     kind = type(action_space).__name__          # a2c_common.py:1211-1224
@@ -134,13 +140,12 @@ class DiscreteModel(FlatParamModel):
                 for i in range(len(self.cnn.layers))]
 
     def _init_like_reference(self, mlp_init):
-        """A2CBuilder.Network.__init__ (network_builder.py:226-341) on torch's global generator, draw for draw: each Conv2d and Linear
+        """A2CBuilder.Network.__init__ (network_builder.py:226-341) on torch's global generator, draw for draw: each Conv2d / Conv1d and Linear
         is constructed (torch's own init) in registration order, _calc_input_size draws its probe frame between the conv trunks and
         the MLPs, then the init loop applies the cnn initializer to every conv weight and the mlp initializer to every linear weight
         (a no-op for 'default'), zeroing every bias."""
         nn = torch.nn
-        convs = [nn.Conv2d(shp[1], shp[0], (shp[2], shp[3]), stride=g[3], padding=g[4]) for _ in range(2 if self.separate else 1)
-                 for shp, g in self.cnn.layers]
+        convs = [self.cnn.module(l) for _ in range(2 if self.separate else 1) for l in range(len(self.cnn.layers))]
         torch.rand(1, *self.cnn.in_shape)
         lins, n_trunks = [], 2 if self.separate else 1
         for _ in range(n_trunks):
@@ -205,41 +210,88 @@ class DiscreteModel(FlatParamModel):
 
 
 class _ConvTrunk:
-    """The geometry of a plain ``conv2d`` cnn (network_builder.py:161-181) on a rank-3 observation.  ``in_shape``: the network's
-    (C, H, W) input, the env's (H, W, C) frame transposed when ``permute_input`` (the default, network_builder.py:360-361);
-    ``layers``: ((Cout, C, KH, KW), (C, H, W, stride, pad)) per conv; ``out_shape`` / ``out_size``: the last conv's output and its
-    flattened size, the MLP's input (_calc_input_size)."""
+    """The geometry of a plain ``conv2d`` cnn (network_builder.py:161-181) on a rank-3 observation, or of a ``conv1d`` cnn
+    (network_builder.py _build_cnn1d) on a rank-2 fp32 one, and the kernels each layer runs on.
+
+    conv2d: ``in_shape`` is the network's (C, H, W) input, the env's (H, W, C) frame transposed when ``permute_input`` (the default,
+    network_builder.py:360-361); ``layers``: ((Cout, C, KH, KW), (C, H, W, stride, pad)) per conv.
+    conv1d: ``in_shape`` is the observation as it is, (C, L) = (frames, features) of a frame stack, or (features, frames) with its
+    ``transpose`` (wrappers.BatchedFrameStack; ``permute_input`` only acts on rank-4 batches); ``layers``: ((Cout, C, k), (C, L,
+    stride, pad)) per conv.
+    ``out_shapes``: each conv's output per sample; ``out_shape`` / ``out_size``: the last one and its flattened size, the MLP's input
+    (_calc_input_size)."""
 
     REFUSED = {'conv2d_spatial_softargmax': 'a spatial soft-argmax head', 'conv2d_flatten': 'a flatten layer',
                'coord_conv2d': 'coordinate channels'}
 
     def __init__(self, cnn, obs_shape):
         ctype = cnn.get('type')
-        if ctype != 'conv2d':
-            why = self.REFUSED.get(ctype, 'only plain conv2d is built')
+        if ctype not in ('conv2d', 'conv1d'):
+            why = self.REFUSED.get(ctype, 'only plain conv2d and conv1d are built')
             raise NotImplementedError(f"'cnn' networks of type {ctype!r} ({why}) are not supported by the discrete B200 agent yet")
-        if len(obs_shape) != 3:
+        self.conv1d = ctype == 'conv1d'
+        if self.conv1d and len(obs_shape) != 2:
+            raise NotImplementedError(f"'cnn' networks of type 'conv1d' need a rank-2 Box observation (frames, features) on the discrete "
+                                      f"B200 agent, got shape {tuple(obs_shape)}")
+        if not self.conv1d and len(obs_shape) != 3:
             raise NotImplementedError(f"a 'conv2d' cnn needs a rank-3 Box observation, got shape {tuple(obs_shape)}")
-        self.nhwc = bool(cnn.get('permute_input', True))
+        self.nhwc = not self.conv1d and bool(cnn.get('permute_input', True))
         self.in_shape = (obs_shape[2], obs_shape[0], obs_shape[1]) if self.nhwc else tuple(obs_shape)
         act = cnn.get('activation', 'relu')
         if act not in ops.ACT:
             raise NotImplementedError(f'cnn activation {act}')
         self.act = ops.ACT[act]
         self.initializer = dict(cnn.get('initializer') or {'name': 'default'})
-        self.layers = []
-        C, H, W = self.in_shape
+        self.layers, self.out_shapes = [], []
+        shape = self.in_shape
         for conv in cnn['convs']:
             k, st, pad = conv['kernel_size'], conv['strides'], conv.get('padding', 0)
             if not all(isinstance(v, int) and not isinstance(v, bool) for v in (k, st, pad)) or k < 1 or st < 1 or pad < 0:
-                raise NotImplementedError(f'conv2d kernel_size / strides / padding must be integers, got {k!r} / {st!r} / {pad!r}')
-            Ho, Wo = (H + 2 * pad - k) // st + 1, (W + 2 * pad - k) // st + 1
-            if Ho < 1 or Wo < 1:
-                raise ValueError(f'conv2d kernel {k} does not fit a {H}x{W} input with padding {pad}')
-            self.layers.append(((int(conv['filters']), C, k, k), (C, H, W, st, pad)))
-            C, H, W = int(conv['filters']), Ho, Wo
-        self.out_shape = (C, H, W)
-        self.out_size = C * H * W
+                raise NotImplementedError(f'{ctype} kernel_size / strides / padding must be integers, got {k!r} / {st!r} / {pad!r}')
+            C, spatial = shape[0], shape[1:]
+            out = tuple((n + 2 * pad - k) // st + 1 for n in spatial)
+            if min(out) < 1:
+                raise ValueError(f"{ctype} kernel {k} does not fit a {'x'.join(map(str, spatial))} input with padding {pad}")
+            Cout = int(conv['filters'])
+            self.layers.append(((Cout, C) + (k,) * len(spatial), (C,) + tuple(spatial) + (st, pad)))
+            shape = (Cout,) + out
+            self.out_shapes.append(shape)
+        self.out_shape = shape
+        self.out_size = int(np.prod(shape))
+
+    def module(self, l):
+        """the reference's torch module of conv l (its construction draws torch's default init)"""
+        shp, g = self.layers[l]
+        if self.conv1d:
+            return torch.nn.Conv1d(shp[1], shp[0], shp[2], g[2], g[3])
+        return torch.nn.Conv2d(shp[1], shp[0], (shp[2], shp[3]), stride=g[3], padding=g[4])
+
+    def out_positions(self):
+        """output positions of the last conv per sample: the rows of its weight gradient's implicit GEMM are M times this"""
+        return int(np.prod(self.out_shape[1:]))
+
+    # one layer of the trunk on kernel set k (layerwise.Kernels): src = the first layer's arena reading (rows_per_chunk, chunk_stride,
+    # x_ld, norm_mean, norm_std); later layers read dense activations
+    def fwd(self, k, l, x, lay, y, M, **src):
+        g = self.layers[l][1]
+        if self.conv1d:
+            k.conv1d_fwd(x, lay.W, lay.b, y, g, lay.act, M, **src)
+        elif src:
+            k.conv_fwd(x, lay.W, lay.b, y, g, lay.act, M, nhwc=self.nhwc, **src)
+        else:
+            k.conv_fwd(x, lay.W, lay.b, y, g, lay.act, M)
+
+    def bwd_data(self, k, l, dy, lay, a_prev, dx, act_prev, M):
+        (k.conv1d_bwd_data if self.conv1d else k.conv_bwd_data)(dy, lay.W, a_prev, dx, self.layers[l][1], act_prev, M)
+
+    def bwd_weight(self, k, l, dy, x, dw, db, lay, n_splits, M, split_stride, **src):
+        g = self.layers[l][1]
+        if self.conv1d:
+            k.conv1d_bwd_weight(dy, x, dw, db, lay.W.shape, g, n_splits, M, split_stride, **src)
+        elif src:
+            k.conv_bwd_weight(dy, x, dw, db, lay.W.shape, g, n_splits, M, split_stride, nhwc=self.nhwc, **src)
+        else:
+            k.conv_bwd_weight(dy, x, dw, db, lay.W.shape, g, n_splits, M, split_stride)
 
 
 class DiscretePolicy:
@@ -276,24 +328,18 @@ class DiscretePolicy:
             out = (acts_a[-1], K, acts_c[-1], 1)
         else:
             acts_c, out = None, (acts_a[-1][:, 1:], K + 1, acts_a[-1], K + 1)
-        conv = lambda: [f(M, shp[0], *self._conv_out(g, shp)) for shp, g in m.cnn.layers]   # noqa: E731
+        conv = lambda: [f(M, *shape) for shape in m.cnn.out_shapes]   # noqa: E731
         return acts_a, acts_c, out, conv() if m.cnn else None, conv() if m.cnn and m.separate else None
-
-    @staticmethod
-    def _conv_out(g, shp):
-        C, H, W, st, pad = g
-        return (H + 2 * pad - shp[2]) // st + 1, (W + 2 * pad - shp[3]) // st + 1
 
     def _conv_forward(self, layers, x, acts, M, rows_per_chunk, chunk_stride):
         """acts[l] = act(conv_l(in_l)): in_0 = the observation rows (arena order, normalised), in_l = acts[l - 1]"""
         m = self.model
         for l, lay in enumerate(layers):
-            g = m.cnn.layers[l][1]
             if l == 0:
-                self.kernels.conv_fwd(x, lay.W, lay.b, acts[0], g, lay.act, M, nhwc=m.cnn.nhwc, rows_per_chunk=rows_per_chunk,
-                                      chunk_stride=chunk_stride, x_ld=m.D, norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
+                m.cnn.fwd(self.kernels, 0, x, lay, acts[0], M, rows_per_chunk=rows_per_chunk, chunk_stride=chunk_stride, x_ld=m.D,
+                          norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
             else:
-                self.kernels.conv_fwd(acts[l - 1], lay.W, lay.b, acts[l], g, lay.act, M)
+                m.cnn.fwd(self.kernels, l, acts[l - 1], lay, acts[l], M)
 
     def _forward(self, x, acts_a, acts_c, M, rows_per_chunk=None, chunk_stride=0, conv=(None, None)):
         """the actor MLP into acts_a (its last entry: [value | logits], or the logits with separate trunks), the critic MLP into acts_c;
@@ -375,6 +421,19 @@ class DiscreteA2CAgent(DiscretePolicy, A2CBase):
         D = m.D
         dev = self.device_t
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)   # noqa: E731
+        if self.mixed_precision:
+            # tensor-core weight gradients: a CTA owns a [128 x <=128] tile of dW and a row split; the continuous agent's layer-wise
+            # rule (16 splits at most) keeps enough CTAs per layer while the split partials stay small
+            self.n_splits = max(1, min(16, mb // 512))
+        else:
+            self.n_splits = layerwise.n_splits(mb)
+        # the conv weight gradients split over the output pixels' rows, so they take more split rows than the MLP.  conv2d: they share
+        # `part`, which gets that many rows over every parameter (the leading conv_params columns hold the conv gradients); conv1d: its
+        # MLP input can be tens of millions of weights per trunk (27m_vs_30m: 1024 filters x 285 positions x 256 units), so the conv
+        # gradients get split rows of their own over the conv parameters only, `cpart`, and `part` keeps the MLP's n_splits rows
+        self.conv_splits = layerwise.n_splits(mb * m.cnn.out_positions()) if m.cnn else 0
+        if m.cnn and m.cnn.conv1d:
+            self._check_memory()
         self.obses = torch.zeros(H, N, D, dtype=self.obs_dtype, device=dev)
         self.actions = (torch.zeros(H, N, len(self.head_sizes), dtype=torch.int64, device=dev) if self.head_sizes
                         else torch.zeros(H, N, dtype=torch.int64, device=dev))
@@ -394,18 +453,14 @@ class DiscreteA2CAgent(DiscretePolicy, A2CBase):
         self.r_a, self.r_c, self.r_out, self.r_ka, self.r_kc = self._alloc_rows(N)
         self.t_a, self.t_c, self.t_out, self.t_ka, self.t_kc = self._alloc_rows(mb)
         self.d_a, self.d_c, self.d_out, self.d_ka, self.d_kc = self._alloc_rows(mb)
-        if self.mixed_precision:
-            # tensor-core weight gradients: a CTA owns a [128 x <=128] tile of dW and a row split; the continuous agent's layer-wise
-            # rule (16 splits at most) keeps enough CTAs per layer while the split partials stay small
-            self.n_splits = max(1, min(16, mb // 512))
-        else:
-            self.n_splits = layerwise.n_splits(mb)
         self._init_policy()
         self._repack()
-        # the conv weight gradients split over the output pixels' rows, so they take more split rows than the MLP (the leading
-        # conv_params columns)
-        self.conv_splits = layerwise.n_splits(mb * m.cnn.out_shape[1] * m.cnn.out_shape[2]) if m.cnn else 0
-        self.part = f(max(self.n_splits, self.conv_splits), m.num_params)
+        if m.cnn and m.cnn.conv1d:
+            self.part = f(self.n_splits, m.num_params)
+            self.cpart, self.cpart_stride = f(self.conv_splits, m.conv_params), m.conv_params
+        else:
+            self.part = f(max(self.n_splits, self.conv_splits), m.num_params)
+            self.cpart, self.cpart_stride = self.part, m.num_params
         self.grad = f(m.num_params)
         self.diag_exp_var = f(self.num_minibatches) if self.diag_on else None
         self._diag_clip = []
@@ -427,6 +482,39 @@ class DiscreteA2CAgent(DiscretePolicy, A2CBase):
                                         float(self.gamma), int(bool(rs.log_val)), int(bool(self.value_bootstrap)))
         self._tensors_ready = True
 
+    def init_tensors_bytes(self):
+        """the device memory init_tensors allocates for a conv1d policy, in bytes, buffer by buffer: the gradient, the split partials
+        (`part`, `cpart`) and the bf16 twin of the parameter arena; the conv and MLP activations of the rollout (N rows) and of a
+        minibatch's forward and gradients (two sets of minibatch rows); the observation arena and the [H, N] rollout buffers (int64
+        actions, eight fp32 rows, dones, action masks, valid flags); the fp64 scratch of the observation moments and of the loss, GAE
+        and post-step partials; the per-row episode state.  The model's own arena (parameters and the two Adam moments, 12 bytes per
+        parameter) is allocated when the model is built."""
+        m, H, N, mb, K = self.model, self.horizon_length, self.num_rows, self.minibatch_size, self.actions_num
+        P, Pc = m.num_params, m.conv_params
+        trunks = 2 if m.separate else 1
+        per_row = trunks * sum(int(np.prod(s)) for s in m.cnn.out_shapes) + trunks * sum(m.units) + K + 1
+        heads = len(self.head_sizes) if self.head_sizes else 1
+        f32 = (P * (1 + self.n_splits) + Pc * self.conv_splits + per_row * (N + 2 * mb)
+               + H * N * (m.D + 8 + (1 if self.mask_autoreset_rows else 0)) + N * 8)
+        f64 = (ops.NUM_SMS * 4 * 2 * m.D + ((mb + 255) // 256) * 8 + max(64, (N + 63) // 64) * 8 + ((N + 255) // 256) * 4)
+        u8 = H * N * (8 * heads + 1 + (K if self.use_action_masks else 0))           # int64 actions, dones, masks
+        return 4 * f32 + 8 * f64 + u8 + (2 * P if self.mixed_precision else 0)
+
+    # what an epoch allocates besides init_tensors' buffers (the stats rows, the KL and diagnostics stacks, the caching allocator's
+    # rounding): under 10 MB on an H100 at the corridor and 27m_vs_30m shapes (tools/conv1d_ab.py, counted against the measured peak)
+    TRANSIENT_BYTES = 256 << 20
+
+    def _check_memory(self):
+        """refuse a geometry whose buffers do not fit the device before anything is allocated, rather than failing mid-epoch"""
+        if self.device_t.type != 'cuda':
+            return
+        need = self.init_tensors_bytes() + self.TRANSIENT_BYTES
+        free, total = torch.cuda.mem_get_info(self.device_t)
+        if need > free:
+            raise RuntimeError(f'this conv1d policy needs {need} bytes of device memory for its training buffers ({need / 2**30:.1f} GiB, '
+                               f'{self.model.num_params} parameters, minibatch {self.minibatch_size}) besides its {12 * self.model.num_params} '
+                               f'bytes of parameters and Adam moments; the device has {free} bytes free of {total}')
+
     # =============================================================================== env plumbing (tensor envs on the device)
     def _to_dev(self, x, dtype=None):
         t = x if torch.is_tensor(x) else torch.as_tensor(np.asarray(x))
@@ -434,7 +522,8 @@ class DiscreteA2CAgent(DiscretePolicy, A2CBase):
         return t if dtype is None or t.dtype == dtype else t.to(dtype)
 
     def _obs_rows(self, o):
-        """observations as arena rows: flat fp32, or image frames flattened in the env's layout and kept in the arena's dtype"""
+        """observations as arena rows: flat fp32, or image frames / frame stacks flattened in the env's layout and kept in the arena's
+        dtype"""
         o = o['obs'] if isinstance(o, dict) else o
         if len(self.obs_shape) == 1:
             return self._to_dev(o, torch.float32).contiguous()
@@ -450,19 +539,18 @@ class DiscreteA2CAgent(DiscretePolicy, A2CBase):
 
     # =============================================================================== backward
     def _conv_backward(self, layers, x, acts, grads, M, rows_per_chunk, chunk_stride):
-        """grads[-1] = dL/d(pre-activation of the last conv) in; weight gradients into the leading columns of `part`"""
-        m, P = self.model, self.model.num_params
+        """grads[-1] = dL/d(pre-activation of the last conv) in; weight gradients into the split rows of `cpart` (row stride
+        `cpart_stride`), at the conv parameters' flat offsets"""
+        m, part, stride = self.model, self.cpart, self.cpart_stride
         for l in range(len(layers) - 1, -1, -1):
-            lay, g = layers[l], m.cnn.layers[l][1]
-            k = self.kernels
+            lay = layers[l]
+            dw, db = part[0, lay.w_off:], part[0, lay.b_off:]
             if l == 0:
-                k.conv_bwd_weight(grads[0], x, self.part[0, lay.w_off:], self.part[0, lay.b_off:], lay.W.shape, g, self.conv_splits, M, P,
-                                  nhwc=m.cnn.nhwc, rows_per_chunk=rows_per_chunk, chunk_stride=chunk_stride, x_ld=m.D,
-                                  norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
+                m.cnn.bwd_weight(self.kernels, 0, grads[0], x, dw, db, lay, self.conv_splits, M, stride, rows_per_chunk=rows_per_chunk,
+                                 chunk_stride=chunk_stride, x_ld=m.D, norm_mean=self.obs_norm[0], norm_std=self.obs_norm[1])
             else:
-                k.conv_bwd_weight(grads[l], acts[l - 1], self.part[0, lay.w_off:], self.part[0, lay.b_off:], lay.W.shape, g,
-                                  self.conv_splits, M, P)
-                k.conv_bwd_data(grads[l], lay.W, acts[l - 1], grads[l - 1], g, layers[l - 1].act, M)
+                m.cnn.bwd_weight(self.kernels, l, grads[l], acts[l - 1], dw, db, lay, self.conv_splits, M, stride)
+                m.cnn.bwd_data(self.kernels, l, grads[l], lay, acts[l - 1], grads[l - 1], layers[l - 1].act, M)
 
     # =============================================================================== rollout
     def play_steps(self, u=None):
@@ -561,7 +649,7 @@ class DiscreteA2CAgent(DiscretePolicy, A2CBase):
                                    dx_out=kgrads[-1].view(mb, -1), dx_act=m.cnn.act)
                 self._conv_backward(conv, x, kacts, kgrads, mb, epm, N)
             Pc = m.conv_params
-            ops.reduce_splits(self.part, self.grad, Pc, self.conv_splits, split_stride=P)
+            ops.reduce_splits(self.cpart, self.grad, Pc, self.conv_splits, split_stride=self.cpart_stride)
             ops.reduce_splits(self.part[0, Pc:], self.grad[Pc:], P - Pc, S, split_stride=P)
         else:
             layerwise.backward(self.kernels, m.actor_mlp, x, self.t_a, self.d_a, self.part, P, S, mb, m.D, epm, N, self.obs_norm)

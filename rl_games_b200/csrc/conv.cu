@@ -1,4 +1,5 @@
-// fp32 (CUDA-core) 2-D convolutions of the image trunk: network_builder.py:161-181 (_build_cnn2d, plain conv2d) and its autograd.
+// fp32 (CUDA-core) 2-D convolutions of the image trunk: network_builder.py:161-181 (_build_cnn2d, plain conv2d) and its autograd, and
+// the 1-D convolutions of a frame-stack trunk (_build_cnn1d, nn.Conv1d) as instantiations of the same kernels (ONE_D below).
 // Implicit GEMM: no im2col is materialised; each tile loader computes the input pixel of its (row, k) pair.
 //   fwd  : Y[m, co, p]  = act( b[co] + sum_k X[m](ci, oh*s+kh-pad, ow*s+kw-pad) . W[co, k] )       k = (ci, kh, kw), p = (oh, ow)
 //   dgrad: dX[m, ci, q] = act'(A_prev[m, ci, q]) * sum_{co, kh, kw} dY[m, co, (ih+pad-kh)/s, (iw+pad-kw)/s] . W[co, ci, kh, kw]
@@ -39,12 +40,16 @@ __device__ __forceinline__ float load_in(const T* __restrict__ row, int ci, int 
     return v;
 }
 
+// The kernels are written once, as inlined bodies, and instantiated twice: the 2-D kernels (ONE_D = false) and the 1-D kernels of a
+// conv1d trunk (ONE_D = true: [C, L] rows as H = 1, W = L, KH = 1, KW = k; the zero padding applies to the W axis only, so the H axis
+// has no padding and Ho = 1).
+
 // ---------------- forward: rows = (m, oh, ow), cols = co, reduction k = (ci, kh, kw) ----------------
-template <typename T, bool NHWC>
-__global__ void __launch_bounds__(NT) conv2d_fwd_kernel(
+template <typename T, bool NHWC, bool ONE_D>
+__device__ __forceinline__ void conv_fwd_body(
     const T* __restrict__ X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
     const float* __restrict__ nm, const float* __restrict__ ns,
-    const float* __restrict__ Wt, const float* __restrict__ bias, float* __restrict__ Y, int M, Geo g, int act) {
+    const float* __restrict__ Wt, const float* __restrict__ bias, float* __restrict__ Y, int M, const Geo& g, int act) {
     __shared__ float As[BK][BM + 4];
     __shared__ float Bs[BK][BN + 4];
     const int tid = threadIdx.x;
@@ -68,7 +73,7 @@ __global__ void __launch_bounds__(NT) conv2d_fwd_kernel(
     if (pv) {
         const int m = (int)(gp / HWo), pix = (int)(gp - (int64_t)m * HWo);
         const int oh = pix / g.Wo, ow = pix - oh * g.Wo;
-        ih0 = oh * g.s - g.pad; iw0 = ow * g.s - g.pad;
+        ih0 = oh * g.s - (ONE_D ? 0 : g.pad); iw0 = ow * g.s - g.pad;
         row = X + chunk_row(m, rows_per_chunk, chunk_stride) * x_ld;
     }
     for (int k0 = 0; k0 < K; k0 += BK) {
@@ -116,10 +121,26 @@ __global__ void __launch_bounds__(NT) conv2d_fwd_kernel(
     }
 }
 
+template <typename T, bool NHWC>
+__global__ void __launch_bounds__(NT) conv2d_fwd_kernel(
+    const T* __restrict__ X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
+    const float* __restrict__ nm, const float* __restrict__ ns,
+    const float* __restrict__ Wt, const float* __restrict__ bias, float* __restrict__ Y, int M, Geo g, int act) {
+    conv_fwd_body<T, NHWC, false>(X, rows_per_chunk, chunk_stride, x_ld, nm, ns, Wt, bias, Y, M, g, act);
+}
+
+__global__ void __launch_bounds__(NT) conv1d_fwd_kernel(
+    const float* __restrict__ X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
+    const float* __restrict__ nm, const float* __restrict__ ns,
+    const float* __restrict__ Wt, const float* __restrict__ bias, float* __restrict__ Y, int M, Geo g, int act) {
+    conv_fwd_body<float, false, true>(X, rows_per_chunk, chunk_stride, x_ld, nm, ns, Wt, bias, Y, M, g, act);
+}
+
 // ---------------- dgrad: rows = input pixels (m, ih, iw), cols = ci, reduction r = (co, kh, kw) ----------------
-__global__ void __launch_bounds__(NT) conv2d_dgrad_kernel(
+template <bool ONE_D>
+__device__ __forceinline__ void conv_dgrad_body(
     const float* __restrict__ dY, const float* __restrict__ Wt, const float* __restrict__ A_prev, float* __restrict__ dX,
-    int M, Geo g, int act_prev) {
+    int M, const Geo& g, int act_prev) {
     __shared__ float As[BK][BM + 4];   // gathered dY tile [r][row]
     __shared__ float Bs[BK][BN + 4];   // W tile [r][ci]
     const int tid = threadIdx.x;
@@ -142,7 +163,7 @@ __global__ void __launch_bounds__(NT) conv2d_dgrad_kernel(
     if (pv) {
         const int m = (int)(gp / HW), q = (int)(gp - (int64_t)m * HW);
         const int ih = q / g.W;
-        ihp = ih + g.pad; iwp = q - ih * g.W + g.pad;
+        ihp = ih + (ONE_D ? 0 : g.pad); iwp = q - ih * g.W + g.pad;
         dy = dY + (int64_t)m * g.Cout * HWo;
     }
     for (int r0 = 0; r0 < R; r0 += BK) {
@@ -203,12 +224,24 @@ __global__ void __launch_bounds__(NT) conv2d_dgrad_kernel(
     }
 }
 
+__global__ void __launch_bounds__(NT) conv2d_dgrad_kernel(
+    const float* __restrict__ dY, const float* __restrict__ Wt, const float* __restrict__ A_prev, float* __restrict__ dX,
+    int M, Geo g, int act_prev) {
+    conv_dgrad_body<false>(dY, Wt, A_prev, dX, M, g, act_prev);
+}
+
+__global__ void __launch_bounds__(NT) conv1d_dgrad_kernel(
+    const float* __restrict__ dY, const float* __restrict__ Wt, const float* __restrict__ A_prev, float* __restrict__ dX,
+    int M, Geo g, int act_prev) {
+    conv_dgrad_body<true>(dY, Wt, A_prev, dX, M, g, act_prev);
+}
+
 // ---------------- wgrad: 64 (co) x 64 (k) block tile, 4x4 per thread, rows of split s in slabs of 16 ----------------
-template <typename T, bool NHWC>
-__global__ void __launch_bounds__(NT) conv2d_wgrad_kernel(
+template <typename T, bool NHWC, bool ONE_D>
+__device__ __forceinline__ void conv_wgrad_body(
     const float* __restrict__ dY, const T* __restrict__ X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
     const float* __restrict__ nm, const float* __restrict__ ns, float* __restrict__ dWp, float* __restrict__ dbp,
-    int M, Geo g, int64_t rows_per_split, int64_t split_stride) {
+    int M, const Geo& g, int64_t rows_per_split, int64_t split_stride) {
     __shared__ float As[BK][64 + 4];   // dY slab [row][co]
     __shared__ float Bs[BK][64 + 4];   // X_col slab [row][k]
     const int tid = threadIdx.x;
@@ -240,7 +273,7 @@ __global__ void __launch_bounds__(NT) conv2d_wgrad_kernel(
         if (mv) {
             m = (int)(p / HWo); pix = (int)(p - (int64_t)m * HWo);
             const int oh = pix / g.Wo, ow = pix - oh * g.Wo;
-            ih0 = oh * g.s - g.pad; iw0 = ow * g.s - g.pad;
+            ih0 = oh * g.s - (ONE_D ? 0 : g.pad); iw0 = ow * g.s - g.pad;
         }
         const float* dy = dY + (int64_t)m * g.Cout * HWo + pix;
         const T* row = X + (mv ? chunk_row(m, rows_per_chunk, chunk_stride) * x_ld : 0);
@@ -281,6 +314,21 @@ __global__ void __launch_bounds__(NT) conv2d_wgrad_kernel(
     if (dbp && blockIdx.y == 0 && tid < 64 && n0 + tid < g.Cout) dbp[(int64_t)s * split_stride + n0 + tid] = bsum;
 }
 
+template <typename T, bool NHWC>
+__global__ void __launch_bounds__(NT) conv2d_wgrad_kernel(
+    const float* __restrict__ dY, const T* __restrict__ X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
+    const float* __restrict__ nm, const float* __restrict__ ns, float* __restrict__ dWp, float* __restrict__ dbp,
+    int M, Geo g, int64_t rows_per_split, int64_t split_stride) {
+    conv_wgrad_body<T, NHWC, false>(dY, X, rows_per_chunk, chunk_stride, x_ld, nm, ns, dWp, dbp, M, g, rows_per_split, split_stride);
+}
+
+__global__ void __launch_bounds__(NT) conv1d_wgrad_kernel(
+    const float* __restrict__ dY, const float* __restrict__ X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
+    const float* __restrict__ nm, const float* __restrict__ ns, float* __restrict__ dWp, float* __restrict__ dbp,
+    int M, Geo g, int64_t rows_per_split, int64_t split_stride) {
+    conv_wgrad_body<float, false, true>(dY, X, rows_per_chunk, chunk_stride, x_ld, nm, ns, dWp, dbp, M, g, rows_per_split, split_stride);
+}
+
 // geometry check shared by the entry points: B200RL_OK and the output size, or B200RL_EINVAL
 int make_geo(Geo& g, int C, int H, int W, int Cout, int KH, int KW, int stride, int pad) {
     if (C <= 0 || H <= 0 || W <= 0 || Cout <= 0 || KH <= 0 || KW <= 0 || stride <= 0 || pad < 0) return B200RL_EINVAL;
@@ -289,6 +337,14 @@ int make_geo(Geo& g, int C, int H, int W, int Cout, int KH, int KW, int stride, 
     // every index the kernels form stays in int32 per row and in int64 across rows
     if ((int64_t)C * H * W >= (1ll << 31) || (int64_t)Cout * g.Ho * g.Wo >= (1ll << 31) || (int64_t)C * KH * KW >= (1ll << 31))
         return B200RL_EINVAL;
+    return B200RL_OK;
+}
+
+// the 1-D geometry of a conv1d layer: [C, L] input as H = 1, W = L; kernel 1 x k; Ho = 1, Wo = (L + 2 pad - k) / stride + 1
+int make_geo1d(Geo& g, int C, int L, int Cout, int k, int stride, int pad) {
+    if (C <= 0 || L <= 0 || Cout <= 0 || k <= 0 || stride <= 0 || pad < 0 || L + 2 * pad < k) return B200RL_EINVAL;
+    g = Geo{C, 1, L, Cout, 1, k, stride, pad, 1, (L + 2 * pad - k) / stride + 1};
+    if ((int64_t)C * L >= (1ll << 31) || (int64_t)Cout * g.Wo >= (1ll << 31) || (int64_t)C * k >= (1ll << 31)) return B200RL_EINVAL;
     return B200RL_OK;
 }
 
@@ -356,6 +412,53 @@ B200RL_EXPORT int b200rl_conv2d_bwd_weight_f32(const float* dY, const void* X, i
         if (x_nhwc) conv2d_wgrad_kernel<float, true><<<grid, NT, 0, s>>>(dY, x, rows_per_chunk, chunk_stride, x_ld, norm_mean, norm_std, dW_part, db_part, M, g, rps, split_stride);
         else conv2d_wgrad_kernel<float, false><<<grid, NT, 0, s>>>(dY, x, rows_per_chunk, chunk_stride, x_ld, norm_mean, norm_std, dW_part, db_part, M, g, rps, split_stride);
     }
+    B200RL_LAUNCH_CHECK();
+    return B200RL_OK;
+}
+
+B200RL_EXPORT int b200rl_conv1d_fwd_f32(const float* X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld, const float* norm_mean,
+                                        const float* norm_std, const float* W, const float* b, float* Y, int M, int C, int L, int Cout,
+                                        int k, int stride, int pad, int act, void* stream) {
+    Geo g;
+    if (!X || !W || !Y || M <= 0 || rows_per_chunk <= 0 || make_geo1d(g, C, L, Cout, k, stride, pad) != B200RL_OK) return B200RL_EINVAL;
+    if ((norm_mean == nullptr) != (norm_std == nullptr) || x_ld < (int64_t)C * L) return B200RL_EINVAL;
+    const int64_t P = (int64_t)M * g.Wo;
+    if ((P + BM - 1) / BM >= (1ll << 31)) return B200RL_EINVAL;
+    dim3 grid((unsigned)((P + BM - 1) / BM), (Cout + BN - 1) / BN);
+    conv1d_fwd_kernel<<<grid, NT, 0, as_stream(stream)>>>(X, rows_per_chunk, chunk_stride, x_ld, norm_mean, norm_std, W, b, Y, M, g, act);
+    B200RL_LAUNCH_CHECK();
+    return B200RL_OK;
+}
+
+B200RL_EXPORT int b200rl_conv1d_bwd_data_f32(const float* dY, const float* W, const float* A_prev, float* dX, int M, int C, int L, int Cout,
+                                             int k, int stride, int pad, int act_prev, void* stream) {
+    Geo g;
+    if (!dY || !W || !dX || M <= 0 || make_geo1d(g, C, L, Cout, k, stride, pad) != B200RL_OK) return B200RL_EINVAL;
+    const int64_t P = (int64_t)M * L;
+    if ((P + BM - 1) / BM >= (1ll << 31)) return B200RL_EINVAL;
+    dim3 grid((unsigned)((P + BM - 1) / BM), (C + BN - 1) / BN);
+    conv1d_dgrad_kernel<<<grid, NT, 0, as_stream(stream)>>>(dY, W, A_prev, dX, M, g, act_prev);
+    B200RL_LAUNCH_CHECK();
+    return B200RL_OK;
+}
+
+B200RL_EXPORT int b200rl_conv1d_bwd_weight_f32(const float* dY, const float* X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
+                                               const float* norm_mean, const float* norm_std, float* dW_part, float* db_part,
+                                               int64_t split_stride, int M, int C, int L, int Cout, int k, int stride, int pad,
+                                               int n_splits, void* stream) {
+    Geo g;
+    if (!dY || !X || !dW_part || M <= 0 || rows_per_chunk <= 0 || n_splits <= 0 || n_splits > 65535 ||
+        make_geo1d(g, C, L, Cout, k, stride, pad) != B200RL_OK)
+        return B200RL_EINVAL;
+    if ((norm_mean == nullptr) != (norm_std == nullptr) || x_ld < (int64_t)C * L) return B200RL_EINVAL;
+    const int K = C * k;
+    if (n_splits > 1 && split_stride < (int64_t)Cout * K) return B200RL_EINVAL;
+    const int64_t P = (int64_t)M * g.Wo;
+    int64_t rps = (P + n_splits - 1) / n_splits;
+    rps = ((rps + BK - 1) / BK) * BK;          // splits past the last row write zeros, which the reduction expects
+    dim3 grid((Cout + 63) / 64, (K + 63) / 64, n_splits);
+    conv1d_wgrad_kernel<<<grid, NT, 0, as_stream(stream)>>>(dY, X, rows_per_chunk, chunk_stride, x_ld, norm_mean, norm_std, dW_part, db_part, M,
+                                                            g, rps, split_stride);
     B200RL_LAUNCH_CHECK();
     return B200RL_OK;
 }

@@ -1,4 +1,5 @@
-// bf16 tensor-core (wgmma) 2-D convolutions of the image trunk: the `mixed_precision: True` path of conv.cu's three operations, with
+// bf16 tensor-core (wgmma) 2-D convolutions of the image trunk, and the 1-D convolutions of a frame-stack trunk as instantiations of the
+// same kernel (ONE_D below): the `mixed_precision: True` path of conv.cu's three operations, with
 // the same semantics, the same fp32 NCHW activation / gradient buffers and the same split-partial weight-gradient format.  Precision
 // contract = gemm_tc.cu's (the reference's bf16 autocast of nn.Conv2d): operands rounded to bf16 while they are staged into shared
 // memory, fp32 accumulation in registers, fp32 bias / activation / outputs.
@@ -92,7 +93,8 @@ __device__ __forceinline__ void item_rc(int i, int& r, int& cg) {
     r = (i & 7) | ((i >> 6) << 3);
 }
 
-template <int MODE, typename T>
+// ONE_D (a conv1d layer: H = 1, KH = 1): the zero padding applies to the W axis only
+template <int MODE, typename T, bool ONE_D>
 __device__ __forceinline__ RowInfo row_a(const ConvArgs& p, int64_t gr) {
     const Geo& g = p.g;
     RowInfo ri{nullptr, 0, 0, 0, gr < p.Mo};
@@ -101,15 +103,15 @@ __device__ __forceinline__ RowInfo row_a(const ConvArgs& p, int64_t gr) {
         const int HWo = g.Ho * g.Wo;
         const int m = (int)(gr / HWo), pix = (int)(gr - (int64_t)m * HWo), oh = pix / g.Wo, ow = pix - oh * g.Wo;
         ri.p = static_cast<const T*>(p.X) + chunk_row(m, p.rows_per_chunk, p.chunk_stride) * p.x_ld;
-        ri.u = oh * g.s - g.pad; ri.v = ow * g.s - g.pad;
+        ri.u = oh * g.s - (ONE_D ? 0 : g.pad); ri.v = ow * g.s - g.pad;
     } else if constexpr (MODE == MODE_DGRAD) {        // input pixel (m, ih, iw): its sample's dY and its padded position
         const int HW = g.H * g.W;
         const int m = (int)(gr / HW), q = (int)(gr - (int64_t)m * HW), ih = q / g.W;
         ri.p = p.dY + (int64_t)m * g.Cout * g.Ho * g.Wo;
-        ri.u = ih + g.pad; ri.v = q - ih * g.W + g.pad;
+        ri.u = ih + (ONE_D ? 0 : g.pad); ri.v = q - ih * g.W + g.pad;
     } else {                                          // reduction column k = (ci, kh, kw)
         const Idx3 x = idx3(gr, g.KH, g.KW);
-        ri.u = x.a; ri.v = x.b - g.pad; ri.w = x.c - g.pad;
+        ri.u = x.a; ri.v = x.b - (ONE_D ? 0 : g.pad); ri.w = x.c - g.pad;
     }
     return ri;
 }
@@ -206,7 +208,9 @@ __device__ __forceinline__ uint4 gather_b(const RowInfo& ri, int64_t r0, int64_t
     return pack8_bf16(f);
 }
 
-template <int MODE, typename T, bool NHWC, int BN>
+// instantiated for the 2-D convolutions (ONE_D = false) and the 1-D convolutions of a conv1d trunk (ONE_D = true: [C, L] fp32 rows as
+// H = 1, W = L, KH = 1, KW = k)
+template <int MODE, typename T, bool NHWC, int BN, bool ONE_D>
 __global__ void __launch_bounds__(GT, 1) conv_tc_kernel(const ConvArgs p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     constexpr int IA = BM * 8 / GT, IB = BN * 8 / GT;          // chunks per thread of the A / B tile
@@ -219,7 +223,7 @@ __global__ void __launch_bounds__(GT, 1) conv_tc_kernel(const ConvArgs p) {
     const int n_slabs = (int)((r_end - r_begin + SLAB - 1) / SLAB);
     RowInfo ra[IA], rb[IB];
 #pragma unroll
-    for (int it = 0; it < IA; ++it) { int r, cg; item_rc(tid + it * GT, r, cg); ra[it] = row_a<MODE, T>(p, m0 + r); }
+    for (int it = 0; it < IA; ++it) { int r, cg; item_rc(tid + it * GT, r, cg); ra[it] = row_a<MODE, T, ONE_D>(p, m0 + r); }
 #pragma unroll
     for (int it = 0; it < IB; ++it) { int r, cg; item_rc(tid + it * GT, r, cg); rb[it] = row_b<MODE>(p, n0 + r); }
     uint4 va[IA], vb[IB];
@@ -325,29 +329,38 @@ int make_geo(Geo& g, int C, int H, int W, int Cout, int KH, int KW, int stride, 
     return B200RL_OK;
 }
 
-template <int MODE, typename T, bool NHWC, int BN>
+// the 1-D geometry of a conv1d layer (conv.cu's): [C, L] input as H = 1, W = L; kernel 1 x k; Ho = 1
+int make_geo1d(Geo& g, int C, int L, int Cout, int k, int stride, int pad) {
+    if (C <= 0 || L <= 0 || Cout <= 0 || k <= 0 || stride <= 0 || pad < 0 || L + 2 * pad < k) return B200RL_EINVAL;
+    g = Geo{C, 1, L, Cout, 1, k, stride, pad, 1, (L + 2 * pad - k) / stride + 1};
+    if ((int64_t)C * L >= (1ll << 31) || (int64_t)Cout * g.Wo >= (1ll << 31) || (int64_t)C * k >= (1ll << 31)) return B200RL_EINVAL;
+    return B200RL_OK;
+}
+
+template <int MODE, typename T, bool NHWC, int BN, bool ONE_D>
 int launch_t(const ConvArgs& a, dim3 grid, void* stream) {
+    auto kernel = conv_tc_kernel<MODE, T, NHWC, BN, ONE_D>;
     static bool raised = false;
     if (!raised) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<MODE, T, NHWC, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES);
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES);
         if (e != cudaSuccess) return (int)e;
         raised = true;
     }
-    conv_tc_kernel<MODE, T, NHWC, BN><<<grid, GT, SMEM_BYTES, as_stream(stream)>>>(a);
+    kernel<<<grid, GT, SMEM_BYTES, as_stream(stream)>>>(a);
     B200RL_LAUNCH_CHECK();
     return B200RL_OK;
 }
 
 // output columns per CTA: the narrowest wgmma tile that holds the layer's columns, 128 past 64
-template <int MODE, typename T, bool NHWC>
+template <int MODE, typename T, bool NHWC, bool ONE_D = false>
 int launch(const ConvArgs& a, int grid_z, void* stream) {
     const int bn = a.No <= 32 ? 32 : a.No <= 64 ? 64 : 128;
     const int64_t gx = (a.Mo + BM - 1) / BM, gy = (a.No + bn - 1) / bn;
     if (gx >= (1ll << 31) || gy > 65535 || grid_z > 65535) return B200RL_EUNSUPPORTED;
     const dim3 grid((unsigned)gx, (unsigned)gy, (unsigned)grid_z);
-    if (bn == 32) return launch_t<MODE, T, NHWC, 32>(a, grid, stream);
-    if (bn == 64) return launch_t<MODE, T, NHWC, 64>(a, grid, stream);
-    return launch_t<MODE, T, NHWC, 128>(a, grid, stream);
+    if (bn == 32) return launch_t<MODE, T, NHWC, 32, ONE_D>(a, grid, stream);
+    if (bn == 64) return launch_t<MODE, T, NHWC, 64, ONE_D>(a, grid, stream);
+    return launch_t<MODE, T, NHWC, 128, ONE_D>(a, grid, stream);
 }
 
 template <int MODE>
@@ -402,4 +415,46 @@ B200RL_EXPORT int b200rl_conv2d_bwd_weight_tc(const float* dY, const void* X, in
     const int64_t rps = (a.R + n_splits - 1) / n_splits;
     a.rows_per_split = ((rps + SLAB - 1) / SLAB) * SLAB;       // trailing splits may be empty: they write zeros, which the reducer expects
     return launch_src<MODE_WGRAD>(a, x_u8, x_nhwc, n_splits, stream);
+}
+
+B200RL_EXPORT int b200rl_conv1d_fwd_tc(const float* X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld, const float* norm_mean,
+                                       const float* norm_std, const void* W_bf16, const float* b, float* Y, int M, int C, int L, int Cout,
+                                       int k, int stride, int pad, int act, void* stream) {
+    ConvArgs a{};
+    if (!X || !W_bf16 || !Y || M <= 0 || rows_per_chunk <= 0 || make_geo1d(a.g, C, L, Cout, k, stride, pad) != B200RL_OK)
+        return B200RL_EINVAL;
+    if ((norm_mean == nullptr) != (norm_std == nullptr) || x_ld < (int64_t)C * L) return B200RL_EINVAL;
+    a.X = X; a.rows_per_chunk = dense_or(rows_per_chunk, M); a.chunk_stride = chunk_stride; a.x_ld = x_ld; a.nm = norm_mean; a.ns = norm_std;
+    a.Wb = static_cast<const __nv_bfloat16*>(W_bf16);
+    a.w_vec = ((int64_t)C * k) % 8 == 0 && (reinterpret_cast<uintptr_t>(W_bf16) & 15) == 0;
+    a.bias = b; a.Y = Y; a.act = act; a.M = M;
+    a.Mo = (int64_t)M * a.g.Wo; a.No = Cout; a.R = (int64_t)C * k;
+    return launch<MODE_FWD, float, false, true>(a, 1, stream);
+}
+
+B200RL_EXPORT int b200rl_conv1d_bwd_data_tc(const float* dY, const void* W_bf16, const float* A_prev, float* dX, int M, int C, int L,
+                                            int Cout, int k, int stride, int pad, int act_prev, void* stream) {
+    ConvArgs a{};
+    if (!dY || !W_bf16 || !dX || M <= 0 || make_geo1d(a.g, C, L, Cout, k, stride, pad) != B200RL_OK) return B200RL_EINVAL;
+    a.dY = dY; a.Wb = static_cast<const __nv_bfloat16*>(W_bf16); a.A_prev = A_prev; a.dX = dX; a.act_prev = act_prev; a.M = M;
+    a.Mo = (int64_t)M * L; a.No = C; a.R = (int64_t)Cout * k;
+    return launch<MODE_DGRAD, float, false, true>(a, 1, stream);
+}
+
+B200RL_EXPORT int b200rl_conv1d_bwd_weight_tc(const float* dY, const float* X, int rows_per_chunk, int64_t chunk_stride, int64_t x_ld,
+                                              const float* norm_mean, const float* norm_std, float* dW_part, float* db_part,
+                                              int64_t split_stride, int M, int C, int L, int Cout, int k, int stride, int pad,
+                                              int n_splits, void* stream) {
+    ConvArgs a{};
+    if (!dY || !X || !dW_part || M <= 0 || rows_per_chunk <= 0 || n_splits <= 0 || make_geo1d(a.g, C, L, Cout, k, stride, pad) != B200RL_OK)
+        return B200RL_EINVAL;
+    if ((norm_mean == nullptr) != (norm_std == nullptr) || x_ld < (int64_t)C * L) return B200RL_EINVAL;
+    const int64_t K = (int64_t)C * k;
+    if (n_splits > 1 && split_stride < (int64_t)Cout * K) return B200RL_EINVAL;
+    a.X = X; a.rows_per_chunk = dense_or(rows_per_chunk, M); a.chunk_stride = chunk_stride; a.x_ld = x_ld; a.nm = norm_mean; a.ns = norm_std;
+    a.dY = dY; a.dW = dW_part; a.db = db_part; a.split_stride = split_stride; a.M = M;
+    a.Mo = K; a.No = Cout; a.R = (int64_t)M * a.g.Wo;
+    const int64_t rps = (a.R + n_splits - 1) / n_splits;
+    a.rows_per_split = ((rps + SLAB - 1) / SLAB) * SLAB;       // trailing splits may be empty: they write zeros, which the reducer expects
+    return launch<MODE_WGRAD, float, false, true>(a, n_splits, stream);
 }

@@ -25,7 +25,8 @@ def n_splits(M):
 
 
 class Kernels:
-    """The three layer GEMMs of one precision, and the three convolutions of an image trunk: fp32, or the tensor cores with weight
+    """The three layer GEMMs of one precision, and the three convolutions of an image trunk (conv2d) and of a frame-stack trunk (conv1d):
+    fp32, or the tensor cores with weight
     operands read from a bf16 twin of the fp32 arena, ``bf16_arena = (fp32 arena, bf16 arena)``, in the forward and the data gradient
     (the tensor-core convs need the twin).  The ``ops`` functions are looked up when the set is built, so that a substitute installed on
     ``ops`` before an agent is built is what runs."""
@@ -34,6 +35,7 @@ class Kernels:
         if not tc:
             self.fwd, self.bwd_data, self.bwd_weight = ops.linear_fwd, ops.linear_bwd_data, ops.linear_bwd_weight
             self.conv_fwd, self.conv_bwd_data, self.conv_bwd_weight = ops.conv2d_fwd, ops.conv2d_bwd_data, ops.conv2d_bwd_weight
+            self.conv1d_fwd, self.conv1d_bwd_data, self.conv1d_bwd_weight = ops.conv1d_fwd, ops.conv1d_bwd_data, ops.conv1d_bwd_weight
             return
         self.fwd = functools.partial(ops.linear_fwd_tc, bf16_arena=bf16_arena)
         self.bwd_data = functools.partial(ops.linear_bwd_data_tc, bf16_arena=bf16_arena)
@@ -41,6 +43,9 @@ class Kernels:
         self.conv_fwd = functools.partial(ops.conv2d_fwd_tc, bf16_arena=bf16_arena)
         self.conv_bwd_data = functools.partial(ops.conv2d_bwd_data_tc, bf16_arena=bf16_arena)
         self.conv_bwd_weight = ops.conv2d_bwd_weight_tc
+        self.conv1d_fwd = functools.partial(ops.conv1d_fwd_tc, bf16_arena=bf16_arena)
+        self.conv1d_bwd_data = functools.partial(ops.conv1d_bwd_data_tc, bf16_arena=bf16_arena)
+        self.conv1d_bwd_weight = ops.conv1d_bwd_weight_tc
 
 
 def forward(k, layers, x, acts, M, x_ld, rows_per_chunk=None, chunk_stride=0, norm=(None, None)):

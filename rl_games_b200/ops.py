@@ -303,6 +303,63 @@ def conv2d_bwd_weight_tc(dY, X, dW_part, db_part, W_shape, geo, n_splits, M, spl
           'conv2d_bwd_weight_tc')
 
 
+def _conv1d_f32(X):
+    if X.dtype != torch.float32:
+        raise TypeError(f'conv1d input dtype {X.dtype}: float32')
+    return ptr(X)
+
+
+def conv1d_fwd(X, W, b, Y, geo, act, M, rows_per_chunk=None, chunk_stride=0, x_ld=None, norm_mean=None, norm_std=None):
+    """Y[M, Cout, Lo] = act(conv1d(norm(X)) + b); geo = (C, L, stride, pad) of the input, W: [Cout, C, k]"""
+    C, L, st, pad = geo
+    Cout, _, k = W.shape
+    check(lib.b200rl_conv1d_fwd_f32(_conv1d_f32(X), M if rows_per_chunk is None else rows_per_chunk, chunk_stride,
+                                    C * L if x_ld is None else x_ld, ptr(norm_mean), ptr(norm_std), ptr(W), ptr(b), ptr(Y), M, C, L, Cout, k,
+                                    st, pad, act, _stream()), 'conv1d_fwd')
+
+
+def conv1d_bwd_data(dY, W, A_prev, dX, geo, act_prev, M):
+    """dX[M, C, L] = conv1d^T(dY, W) * act'(A_prev)"""
+    C, L, st, pad = geo
+    Cout, _, k = W.shape
+    check(lib.b200rl_conv1d_bwd_data_f32(ptr(dY), ptr(W), ptr(A_prev), ptr(dX), M, C, L, Cout, k, st, pad, act_prev, _stream()),
+          'conv1d_bwd_data')
+
+
+def conv1d_bwd_weight(dY, X, dW_part, db_part, W_shape, geo, n_splits, M, split_stride, rows_per_chunk=None, chunk_stride=0, x_ld=None,
+                      norm_mean=None, norm_std=None):
+    C, L, st, pad = geo
+    Cout, _, k = W_shape
+    check(lib.b200rl_conv1d_bwd_weight_f32(ptr(dY), _conv1d_f32(X), M if rows_per_chunk is None else rows_per_chunk, chunk_stride,
+                                           C * L if x_ld is None else x_ld, ptr(norm_mean), ptr(norm_std), ptr(dW_part), ptr(db_part),
+                                           split_stride, M, C, L, Cout, k, st, pad, n_splits, _stream()), 'conv1d_bwd_weight')
+
+
+def conv1d_fwd_tc(X, W, b, Y, geo, act, M, rows_per_chunk=None, chunk_stride=0, x_ld=None, norm_mean=None, norm_std=None, bf16_arena=None):
+    """conv1d_fwd on the tensor cores (bf16 operands, fp32 accumulate); weights from the bf16 twin"""
+    C, L, st, pad = geo
+    Cout, _, k = W.shape
+    check(lib.b200rl_conv1d_fwd_tc(_conv1d_f32(X), M if rows_per_chunk is None else rows_per_chunk, chunk_stride,
+                                   C * L if x_ld is None else x_ld, ptr(norm_mean), ptr(norm_std), _conv_bf16_ptr(W, bf16_arena), ptr(b),
+                                   ptr(Y), M, C, L, Cout, k, st, pad, act, _stream()), 'conv1d_fwd_tc')
+
+
+def conv1d_bwd_data_tc(dY, W, A_prev, dX, geo, act_prev, M, bf16_arena=None):
+    C, L, st, pad = geo
+    Cout, _, k = W.shape
+    check(lib.b200rl_conv1d_bwd_data_tc(ptr(dY), _conv_bf16_ptr(W, bf16_arena), ptr(A_prev), ptr(dX), M, C, L, Cout, k, st, pad, act_prev,
+                                        _stream()), 'conv1d_bwd_data_tc')
+
+
+def conv1d_bwd_weight_tc(dY, X, dW_part, db_part, W_shape, geo, n_splits, M, split_stride, rows_per_chunk=None, chunk_stride=0, x_ld=None,
+                         norm_mean=None, norm_std=None):
+    C, L, st, pad = geo
+    Cout, _, k = W_shape
+    check(lib.b200rl_conv1d_bwd_weight_tc(ptr(dY), _conv1d_f32(X), M if rows_per_chunk is None else rows_per_chunk, chunk_stride,
+                                          C * L if x_ld is None else x_ld, ptr(norm_mean), ptr(norm_std), ptr(dW_part), ptr(db_part),
+                                          split_stride, M, C, L, Cout, k, st, pad, n_splits, _stream()), 'conv1d_bwd_weight_tc')
+
+
 def moments_update_u8(x, D, rows_per_chunk, n_chunks, chunk_stride, mean, var, count, mean_f32, std_f32, eps=1e-5):
     """moments_update of uint8 rows, read as x / 255"""
     check(lib.b200rl_moments_update_u8_f64(ptr(x), D, rows_per_chunk, n_chunks, chunk_stride, ptr(mean), ptr(var), ptr(count),
