@@ -379,8 +379,7 @@ int b200rl_mask_inv_counts_f32(const float* mask, int H, int N, int envs_per_mb,
 int b200rl_loss_partial_stride(void);
 
 /* ---------------------------------------------------------------------------------------------
- * Categorical (discrete-action) policy head -- SURVEY 8a row a15.  NOT YET RUN ON HARDWARE (see csrc/discrete.cu): the CPU
- * oracle (oracle/ppo_discrete_oracle.py) is pinned to the reference; these kernels are validated in the next round.
+ * Categorical (discrete-action) policy head -- SURVEY 8a row a15 (csrc/discrete.cu).
  *  b200rl_categorical_sample_f32: rollout head (models.py:95-125 eval branch; CategoricalMasked distributions.py:23-44):
  *    logits [N, ld] (K used), value_raw [N*value_ld], optional action_masks uint8 [N, K], one uniform per row from u_tape [N] or
  *    Philox(seed, *rng_epoch_dev, step_index, row); action = #{k : cdf_k <= u} clamped to the last action with p > 0;
@@ -393,6 +392,23 @@ int b200rl_loss_partial_stride(void);
  *    mean(a) + 0.5 critic_coef mean(c) - entropy_coef mean(H) (masked means when mask / inv_count_dev are given), and
  *    per-block partial rows of 8 doubles {w*a, w*c, w*H, w*kl, mask, mask*clipped, w, 0}.  Arena tensors (actions, action_masks,
  *    old_values_n, returns_n, old_neglogp, advs_n, mask) are addressed as chunk_row(m, rows_per_chunk, chunk_stride).
+ *  These two (and b200rl_categorical_argmax_f32) are the NARROW kernels, one thread per row: they take layouts of at most 8 heads of at
+ *  most 64 actions each and refuse every other layout with B200RL_EINVAL.
+ *
+ *  The _wide_ entry points take any layout: any number of heads (n_heads), any head size, K + 1 logits per row up to the int range.
+ *  Arguments and outputs are those of the narrow entry point of the same name, plus head_offsets_dev: a DEVICE int32 table
+ *  [n_heads + 1] of head offsets (0, K_0, K_0 + K_1, ..., K), which must describe the same layout as head_sizes_host (the host copy
+ *  is what the entry point checks); NULL when n_heads = 0 (one head of K).  One CTA per row, one warp per head (warp w of
+ *  W = min(n_heads, 8) takes heads w, w + W, ...); a row's neglogp and entropy are summed per warp in head order, then over the warps in
+ *  warp order, so two runs give the same bits.  Masked logits count as -1e8, as in the narrow kernels.
+ *   - sample: the cdf of a head is summed 32 actions at a time: cdf_k = carry + S(k), S the inclusive Hillis-Steele scan of p over the
+ *     chunk [32c, 32c + 32) (steps d = 1, 2, 4, 8, 16: x_l += x_{l-d} for l >= d) and carry the cdf at the previous chunk's last action
+ *     (0 before the first); this order decides which action a uniform on a cdf boundary picks.  Philox counter of head j of row e:
+ *     ctr_lo = e | (j >> 3) << 32, ctr_hi = epoch << 20 | step << 4 | (8 + (j & 7)); for j < 8 this is the narrow sampler's counter,
+ *     and for j >= 8 the high word of ctr_lo is non-zero, which no other policy sampler uses (rows < 2^31).  No values_only mode: the
+ *     narrow entry point serves it for every layout.
+ *   - loss: partial rows are one per ROW (M rows of 8 doubles, same columns); *n_blocks_out_host = M, max_partials >= M.  d_logits
+ *     doubles as the kernel's scratch between its two passes: it must not alias the logits.
  * ------------------------------------------------------------------------------------------- */
 typedef struct b200rl_cat_loss_cfg {
     float e_clip, critic_coef, entropy_coef;
@@ -412,6 +428,20 @@ int b200rl_categorical_loss_f32(const float* logits, int ld, int K, int n_heads,
                                 int rows_per_chunk, int64_t chunk_stride, int M, const b200rl_cat_loss_cfg* cfg_host,
                                 const float* inv_count_dev, float* d_logits, int d_ld, float* d_value, int dv_ld,
                                 double* partials, int max_partials, int* n_blocks_out_host, void* stream);
+int b200rl_categorical_sample_wide_f32(const float* logits, int ld, int K, int n_heads, const int* head_sizes_host,
+                                       const int* head_offsets_dev, const float* value_raw, int value_ld,
+                                       const uint8_t* action_masks, const float* u_tape, uint64_t seed,
+                                       const uint64_t* rng_epoch_dev, uint32_t step_index, const double* vms_mean,
+                                       const double* vms_var, int normalize_value, int64_t* actions, float* neglogp,
+                                       float* values, const uint8_t* dones_cur, uint8_t* dones_out, const float* prev_dones,
+                                       float* valid_out, int N, void* stream);
+int b200rl_categorical_loss_wide_f32(const float* logits, int ld, int K, int n_heads, const int* head_sizes_host,
+                                     const int* head_offsets_dev, const float* values, int value_ld,
+                                     const int64_t* actions, const uint8_t* action_masks, const float* old_values_n,
+                                     const float* returns_n, const float* old_neglogp, const float* advs_n, const float* mask,
+                                     int rows_per_chunk, int64_t chunk_stride, int M, const b200rl_cat_loss_cfg* cfg_host,
+                                     const float* inv_count_dev, float* d_logits, int d_ld, float* d_value, int dv_ld,
+                                     double* partials, int max_partials, int* n_blocks_out_host, void* stream);
 /* Deterministic categorical head of the discrete player (csrc/player.cu; algos_torch/players.py get_action / get_masked_action with
  * is_deterministic): actions_out int64 [N, max(n_heads, 1)] = the per-head argmax of logits [N, ld] (K used; heads laid out as in
  * b200rl_categorical_sample_f32, n_heads = 0 or NULL sizes: one head of K <= 64, else <= 8 heads of <= 64) over the actions the optional
@@ -419,6 +449,11 @@ int b200rl_categorical_loss_f32(const float* logits, int ld, int K, int n_heads,
  * Caller-owned buffers, no allocation, asynchronous on `stream`, graph-capturable. */
 int b200rl_categorical_argmax_f32(const float* logits, int ld, int K, int n_heads, const int* head_sizes_host,
                                   const uint8_t* action_masks, int64_t* actions_out, int N, void* stream);
+/* the same for any layout (head_offsets_dev as in the wide sample / loss entry points): one CTA per row, one warp per head, the same
+ * tie, NaN and all-masked rules */
+int b200rl_categorical_argmax_wide_f32(const float* logits, int ld, int K, int n_heads, const int* head_sizes_host,
+                                       const int* head_offsets_dev, const uint8_t* action_masks, int64_t* actions_out, int N,
+                                       void* stream);
 
 /* Central value with a multi-agent env (agents > 1; central_value.py:224-244).
  *  b200rl_cv_value_broadcast_f32: out[e*agents + a] = denorm(val[e]) for the N envs' critic values val[N] (de-normalised with the value

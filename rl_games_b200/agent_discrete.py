@@ -3,7 +3,7 @@ DiscreteA2CAgent + common/a2c_common.py:1205-1359 DiscreteA2CBase, models.py:62-
 ``discrete`` space, optionally ``separate: True`` actor/critic trunks, optional action masks).
 
 STATUS: parity-green on an H100 (``tests/test_discrete_gpu.py``) against a CPU oracle that is pinned to the reference
-(oracle/ppo_discrete_oracle.py, tests/golden/agent_discrete*.pt).  Everything except the two categorical kernels
+(oracle/ppo_discrete_oracle.py, tests/golden/agent_discrete*.pt).  Everything except the categorical kernels
 (csrc/discrete.cu) reuses the kernels of the continuous path: linear_fwd / linear_bwd_* / reduce_splits (mlp_simt.cu), gae_fused, prepare_batch, moments_update,
 mask_inv_counts (stats.cu, gae.cu), post_step (rollout.cu), adam_step (adam.cu).
 
@@ -14,7 +14,10 @@ tensor cores (csrc/conv_tc.cu, csrc/gemm_tc.cu; the categorical head kernels sta
 twin of the parameter arena refreshed after every optimiser step, weight load and weight broadcast; ``False`` or no key runs the fp32
 kernels above.
 Scope of this first edition: one GPU, eager launches (no CUDA graph), flat Box observations, conv2d frames or conv1d frame stacks, ``Discrete(K)`` or multi-discrete
-``Tuple(Discrete(K_j))`` action spaces (K_j <= 64, <= 8 heads), no RNN, no central value.  The scheduler steps once per MINI-EPOCH on the mean KL like the reference
+``Tuple(Discrete(K_j))`` action spaces of any width, no RNN, no central value.  Layouts of at most 8 heads of at most 64 actions run on
+the one-thread-per-row categorical kernels; every wider layout (Go's ``Discrete(362)``, a chess move encoding's ``Discrete(4672)``, a
+per-cell ``Tuple`` of thousands of heads) runs on the wide kernels, one CTA per row and one warp per head (DESIGN.md §4), and is checked
+against the device's free memory before its buffers are allocated.  The scheduler steps once per MINI-EPOCH on the mean KL like the reference
 (a2c_common.py:1265-1272), which costs one host sync per mini-epoch.
 
 The agent derives from ``a2c_base.A2CBase`` (shared with the continuous agent) and adds the action space, the model, the arena, the
@@ -31,6 +34,9 @@ from .a2c_base import A2CBase
 from .common import make_summary_writer
 from .layerwise import Layer
 from .model import _apply_init, check_network_params, FlatParamModel, _RunningStats
+
+# output columns of one linear layer: the fp32 and tensor-core linear kernels tile them 64 wide on grid.y (at most 65535 CTAs)
+HEAD_MAX_OUTPUTS = 65535 * 64
 
 
 def discrete_spaces(observation_space, action_space, network_params, config):
@@ -54,12 +60,19 @@ def discrete_spaces(observation_space, action_space, network_params, config):
     elif kind == 'Tuple':
         head_sizes = [int(a.n) for a in action_space]
         actions_num, is_multi_discrete = sum(head_sizes), True      # width of the concatenated logits
-        if len(head_sizes) > 8:
-            raise NotImplementedError('more than 8 heads in a multi-discrete space')
     else:
         raise ValueError(f'Unsupported action space type for DiscreteA2CBase: {type(action_space)}')
-    if max(head_sizes or [actions_num]) > 64:
-        raise NotImplementedError('more than 64 actions in one discrete head')
+    # any number of heads of any size: layouts of at most 8 heads of at most 64 actions run on the narrow categorical kernels, every
+    # other layout on the wide ones (ops.categorical_is_wide)
+    if min(head_sizes or [actions_num]) < 1:
+        raise ValueError(f'a discrete action head of 0 actions ({head_sizes or actions_num}) cannot be sampled')
+    if actions_num + 1 > HEAD_MAX_OUTPUTS:
+        raise NotImplementedError(f'{actions_num} logits per row: the [value | logits] head layer has at most {HEAD_MAX_OUTPUTS} outputs '
+                                  f'(the linear kernels put 64 output columns per CTA on a grid axis of 65535)')
+    hl = (network_params.get('mlp') or {}).get('units') or [0]
+    if (actions_num + 1) * int(hl[-1]) >= 2 ** 31:
+        raise NotImplementedError(f'{actions_num} logits per row from {hl[-1]} units: the head layer alone has more parameters than the '
+                                  f'32-bit parameter index of the optimiser kernels covers')
     # True: every conv and linear layer on the bf16 tensor cores (conv_tc.cu, gemm_tc.cu); False or absent: the fp32 kernels
     mixed_precision = bool(config.get('mixed_precision') or False)
     return obs_shape, obs_dtype, head_sizes, actions_num, is_multi_discrete, mixed_precision
@@ -432,7 +445,7 @@ class DiscreteA2CAgent(DiscretePolicy, A2CBase):
         # MLP input can be tens of millions of weights per trunk (27m_vs_30m: 1024 filters x 285 positions x 256 units), so the conv
         # gradients get split rows of their own over the conv parameters only, `cpart`, and `part` keeps the MLP's n_splits rows
         self.conv_splits = layerwise.n_splits(mb * m.cnn.out_positions()) if m.cnn else 0
-        if m.cnn and m.cnn.conv1d:
+        if m.cnn and m.cnn.conv1d or ops.categorical_is_wide(K, self.head_sizes):
             self._check_memory()
         self.obses = torch.zeros(H, N, D, dtype=self.obs_dtype, device=dev)
         self.actions = (torch.zeros(H, N, len(self.head_sizes), dtype=torch.int64, device=dev) if self.head_sizes
@@ -464,7 +477,7 @@ class DiscreteA2CAgent(DiscretePolicy, A2CBase):
         self.grad = f(m.num_params)
         self.diag_exp_var = f(self.num_minibatches) if self.diag_on else None
         self._diag_clip = []
-        self.loss_partials = torch.zeros((mb + 255) // 256, 8, dtype=torch.float64, device=dev)
+        self.loss_partials = torch.zeros(ops.categorical_loss_partial_rows(mb, K, self.head_sizes), 8, dtype=torch.float64, device=dev)
         self.gae_partials = torch.zeros(max(64, (N + 63) // 64), 8, dtype=torch.float64, device=dev)
         self.inv_counts = f(self.num_minibatches) if self.mask_autoreset_rows else None
         # uint8 frames update their statistics without partials (moments_update_u8); fp32 rows need NUM_SMS * 4 partial rows
@@ -483,20 +496,23 @@ class DiscreteA2CAgent(DiscretePolicy, A2CBase):
         self._tensors_ready = True
 
     def init_tensors_bytes(self):
-        """the device memory init_tensors allocates for a conv1d policy, in bytes, buffer by buffer: the gradient, the split partials
-        (`part`, `cpart`) and the bf16 twin of the parameter arena; the conv and MLP activations of the rollout (N rows) and of a
-        minibatch's forward and gradients (two sets of minibatch rows); the observation arena and the [H, N] rollout buffers (int64
-        actions, eight fp32 rows, dones, action masks, valid flags); the fp64 scratch of the observation moments and of the loss, GAE
-        and post-step partials; the per-row episode state.  The model's own arena (parameters and the two Adam moments, 12 bytes per
-        parameter) is allocated when the model is built."""
+        """the device memory init_tensors allocates for a conv1d or a wide-head policy, in bytes, buffer by buffer: the gradient, the
+        split partials (`part`, `cpart`) and the bf16 twin of the parameter arena; the conv and MLP activations (the head's 1 + K
+        columns included) of the rollout (N rows) and of a minibatch's forward and gradients (two sets of minibatch rows); the
+        observation arena and the [H, N] rollout buffers (int64 actions per head, eight fp32 rows, dones, [H, N, K] action masks, valid
+        flags); the fp64 scratch of the observation moments and of the loss (one partial row per minibatch row on the wide kernels),
+        GAE and post-step partials; the per-row episode state.  The model's own arena (parameters and the two Adam moments, 12 bytes
+        per parameter) is allocated when the model is built."""
         m, H, N, mb, K = self.model, self.horizon_length, self.num_rows, self.minibatch_size, self.actions_num
         P, Pc = m.num_params, m.conv_params
         trunks = 2 if m.separate else 1
-        per_row = trunks * sum(int(np.prod(s)) for s in m.cnn.out_shapes) + trunks * sum(m.units) + K + 1
+        conv_row = sum(int(np.prod(s)) for s in m.cnn.out_shapes) if m.cnn else 0
+        per_row = trunks * conv_row + trunks * sum(m.units) + K + 1
         heads = len(self.head_sizes) if self.head_sizes else 1
         f32 = (P * (1 + self.n_splits) + Pc * self.conv_splits + per_row * (N + 2 * mb)
                + H * N * (m.D + 8 + (1 if self.mask_autoreset_rows else 0)) + N * 8)
-        f64 = (ops.NUM_SMS * 4 * 2 * m.D + ((mb + 255) // 256) * 8 + max(64, (N + 63) // 64) * 8 + ((N + 255) // 256) * 4)
+        f64 = (ops.NUM_SMS * 4 * 2 * m.D + ops.categorical_loss_partial_rows(mb, K, self.head_sizes) * 8 + max(64, (N + 63) // 64) * 8
+               + ((N + 255) // 256) * 4)
         u8 = H * N * (8 * heads + 1 + (K if self.use_action_masks else 0))           # int64 actions, dones, masks
         return 4 * f32 + 8 * f64 + u8 + (2 * P if self.mixed_precision else 0)
 
@@ -511,7 +527,8 @@ class DiscreteA2CAgent(DiscretePolicy, A2CBase):
         need = self.init_tensors_bytes() + self.TRANSIENT_BYTES
         free, total = torch.cuda.mem_get_info(self.device_t)
         if need > free:
-            raise RuntimeError(f'this conv1d policy needs {need} bytes of device memory for its training buffers ({need / 2**30:.1f} GiB, '
+            what = 'conv1d' if self.model.cnn and self.model.cnn.conv1d else 'wide-head'
+            raise RuntimeError(f'this {what} policy needs {need} bytes of device memory for its training buffers ({need / 2**30:.1f} GiB, '
                                f'{self.model.num_params} parameters, minibatch {self.minibatch_size}) besides its {12 * self.model.num_params} '
                                f'bytes of parameters and Adam moments; the device has {free} bytes free of {total}')
 

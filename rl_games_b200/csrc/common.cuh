@@ -81,7 +81,9 @@ __device__ __forceinline__ void block_sum_d(double (&v)[NV], double* sm) {
 // ---- Philox4x32-10 (Salmon et al.), counter-based so launches are CUDA-graph replayable ----------
 // Counter layout: ctr_lo = row (env index), ctr_hi = bit fields that must never overlap, or two draws would share a stream.
 //   policy samplers (rollout.cu, mlp_tc.cu, discrete.cu): epoch << 20 | step << 4 | q,  step < 2^16, q < 16:
-//     Gaussian heads q = 0..7 (four normals per q, up to 32 actions), categorical heads q = 8 + j (j < CAT_MAXH = 8)
+//     Gaussian heads q = 0..7 (four normals per q, up to 32 actions), categorical heads q = 8 + j (j < CAT_MAXH = 8); the wide
+//     categorical sampler's head j uses q = 8 + (j & 7) with (j >> 3) in the high word of ctr_lo, which is 0 for every other
+//     policy sampler (rows < 2^31)
 //   synthetic env (rollout.cu synth_env_step_kernel, its own keys): epoch << 20 | step << 10 | q, step < 2^10,
 //     q < 2^9 (feature group of four), bit 9 set for the done draw
 // tests/_philox_ref.py restates this generator and the mappings below bit for bit on the host.

@@ -762,11 +762,51 @@ def _head_table(head_sizes):
     return len(head_sizes), arr
 
 
+# layouts of the one-thread-per-row ("narrow") categorical kernels: at most 8 heads of at most 64 actions; every other layout runs on the
+# wide kernels (one CTA per row, one warp per head).  The choice follows the layout only.
+CAT_NARROW_MAXK, CAT_NARROW_MAXH = 64, 8
+
+
+def categorical_is_wide(K, head_sizes=None):
+    sizes = list(head_sizes) if head_sizes else [K]
+    return len(sizes) > CAT_NARROW_MAXH or max(sizes) > CAT_NARROW_MAXK
+
+
+def categorical_loss_partial_rows(M, K, head_sizes=None):
+    """partial rows categorical_loss writes for M rows: one per 256 rows (narrow kernel), one per row (wide kernel)"""
+    return M if categorical_is_wide(K, head_sizes) else (M + 255) // 256
+
+
+_HEAD_OFFSETS = {}
+
+
+def _head_offsets(head_sizes, device):
+    """the wide kernels' device head table, int32 [n_heads + 1] offsets (None for one head), made once per layout and device so that a
+    CUDA-graph capture of a step that already ran eagerly finds it"""
+    if not head_sizes:
+        return None
+    key = (tuple(int(k) for k in head_sizes), torch.device(device))
+    t = _HEAD_OFFSETS.get(key)
+    if t is None:
+        off = [0]
+        for k in key[0]:
+            off.append(off[-1] + k)
+        t = _HEAD_OFFSETS[key] = torch.tensor(off, dtype=torch.int32, device=device)
+    return t
+
+
 def categorical_sample(logits, ld, K, value_raw, value_ld, action_masks, u_tape, seed, rng_epoch, step_index, vms_mean, vms_var,
                        normalize_value, actions, neglogp, values, dones_cur, dones_out, prev_dones, valid_out, N, values_only=False,
                        head_sizes=None):
     """head_sizes: sizes of the heads of a multi-discrete (Tuple) space (sum = K; actions [N, n_heads], u_tape [n_heads, N]); None = one head"""
     nh, tab = _head_table(head_sizes)
+    if not values_only and categorical_is_wide(K, head_sizes):
+        check(lib.b200rl_categorical_sample_wide_f32(
+            ptr(logits), ld, K, nh, None if tab is None else ctypes.addressof(tab), ptr(_head_offsets(head_sizes, logits.device)),
+            ptr(value_raw), value_ld, ptr(action_masks), ptr(u_tape), seed, ptr(rng_epoch), step_index, ptr(vms_mean), ptr(vms_var),
+            int(normalize_value), ptr(actions), ptr(neglogp), ptr(values), ptr(dones_cur), ptr(dones_out), ptr(prev_dones), ptr(valid_out), N,
+            _stream()), 'categorical_sample_wide')
+        return
     check(lib.b200rl_categorical_sample_f32(ptr(logits), ld, K, nh, None if tab is None else ctypes.addressof(tab), ptr(value_raw), value_ld,
                                             ptr(action_masks), ptr(u_tape), seed, ptr(rng_epoch), step_index, ptr(vms_mean), ptr(vms_var),
                                             int(normalize_value), ptr(actions), ptr(neglogp), ptr(values), ptr(dones_cur), ptr(dones_out),
@@ -776,19 +816,27 @@ def categorical_sample(logits, ld, K, value_raw, value_ld, action_masks, u_tape,
 def categorical_argmax(logits, ld, K, action_masks, actions_out, N, head_sizes=None):
     """deterministic discrete action (csrc/player.cu): per-head argmax of the allowed logits into actions_out int64 [N, n_heads]"""
     nh, tab = _head_table(head_sizes)
+    if categorical_is_wide(K, head_sizes):
+        check(lib.b200rl_categorical_argmax_wide_f32(ptr(logits), ld, K, nh, None if tab is None else ctypes.addressof(tab),
+                                                     ptr(_head_offsets(head_sizes, logits.device)), ptr(action_masks), ptr(actions_out), N,
+                                                     _stream()), 'categorical_argmax_wide')
+        return
     check(lib.b200rl_categorical_argmax_f32(ptr(logits), ld, K, nh, None if tab is None else ctypes.addressof(tab), ptr(action_masks),
                                             ptr(actions_out), N, _stream()), 'categorical_argmax')
 
 
 def categorical_loss(logits, ld, K, values, value_ld, actions, action_masks, old_values_n, returns_n, old_neglogp, advs_n, mask,
                      rows_per_chunk, chunk_stride, M, cfg, inv_count, d_logits, d_ld, d_value, dv_ld, partials, head_sizes=None):
+    """partials: categorical_loss_partial_rows(M, K, head_sizes) rows of 8 doubles at least; returns the number written"""
     nb = ctypes.c_int(0)
     nh, tab = _head_table(head_sizes)
-    check(lib.b200rl_categorical_loss_f32(ptr(logits), ld, K, nh, None if tab is None else ctypes.addressof(tab), ptr(values), value_ld,
-                                          ptr(actions), ptr(action_masks), ptr(old_values_n), ptr(returns_n), ptr(old_neglogp), ptr(advs_n),
-                                          ptr(mask), rows_per_chunk, chunk_stride, M, ctypes.addressof(cfg), ptr(inv_count), ptr(d_logits),
-                                          d_ld, ptr(d_value), dv_ld, ptr(partials), partials.shape[0], ctypes.addressof(nb), _stream()),
-          'categorical_loss')
+    wide = categorical_is_wide(K, head_sizes)
+    fn = lib.b200rl_categorical_loss_wide_f32 if wide else lib.b200rl_categorical_loss_f32
+    table = (nh, None if tab is None else ctypes.addressof(tab)) + ((ptr(_head_offsets(head_sizes, logits.device)),) if wide else ())
+    check(fn(ptr(logits), ld, K, *table, ptr(values), value_ld, ptr(actions), ptr(action_masks), ptr(old_values_n), ptr(returns_n),
+             ptr(old_neglogp), ptr(advs_n), ptr(mask), rows_per_chunk, chunk_stride, M, ctypes.addressof(cfg), ptr(inv_count), ptr(d_logits),
+             d_ld, ptr(d_value), dv_ld, ptr(partials), partials.shape[0], ctypes.addressof(nb), _stream()),
+          'categorical_loss_wide' if wide else 'categorical_loss')
     return nb.value
 
 

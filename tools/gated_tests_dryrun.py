@@ -60,11 +60,11 @@ class _Any:
 pytest.approx = lambda *a, **k: _Any()
 mods = ['test_agent_gpu', 'test_kernels_gpu', 'test_mlp_tc_gpu', 'test_tc_faithful_gpu', 'test_gemm_tc_gpu', 'test_discrete_gpu', 'test_cv_gpu', 'test_tc_gpu', 'test_zz_env_adapters_gpu',
         'test_heads_action_dims_gpu', 'test_lstm_grad_gpu', 'test_cnn_gpu', 'test_conv_tc_gpu',
-        'test_layer_census_gpu', 'test_conv1d_gpu']
+        'test_layer_census_gpu', 'test_conv1d_gpu', 'test_cat_wide_gpu']
 # tests that need a real device object even to get going (CUDA generator, IPC allocation, the capture stream of a CUDA-graphed player
 # step): nothing to learn from them here
 NEEDS_DEVICE = {'test_fused_allreduce_adam_world1_matches_adam_step', 'test_gae_full_size_properties',
-                'test_conv1d_player_matches_the_reference_player'}
+                'test_conv1d_player_matches_the_reference_player', 'test_wide_player_plays_the_reference_rule_on_a_trained_checkpoint'}
 bad = 0
 for mn in mods:
     m = __import__(mn)
